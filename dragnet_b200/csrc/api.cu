@@ -40,6 +40,7 @@ namespace {
 
 const size_t RING_SLOTS = 3;
 const size_t CARRY_ROOM = (size_t)DNG_MAXREC + 4096;	/* room before a chunk */
+const size_t DNG_ARENA_MAX = (size_t)2 << 30;	/* largest DNG_ARENA_BYTES */
 
 size_t env_size(const char *name, size_t dflt)
 {
@@ -201,6 +202,7 @@ struct dng_scan {
 					 * the tally cache needs the shared memory */
 	unsigned long long seen_over = 0, seen_aggr = 0;
 	bool f_probed = false;
+	bool f_forced = false;		/* DNG_F_WARPS chose f_nt: not remembered */
 	u32 f_nsl = 13;			/* 16-byte units per lane slice */
 	double mean_line = 224;		/* of the sample the templates came from */
 	u32 f_smem_max = 0;		/* dynamic shared memory a CTA may ask for */
@@ -288,6 +290,10 @@ static unsigned long long fplan_hash(const FPlan &F)
 
 static void fnt_remember(const dng_scan *s)
 {
+	/* a count forced by DNG_F_WARPS says nothing about the plan, and would
+	 * otherwise stay in force for every later scan of it in this process */
+	if (s->f_forced)
+		return;
 	std::lock_guard<std::mutex> g(g_fnt_mu);
 	g_fnt_memo[fplan_hash(s->fplan)] = s->f_nt;
 }
@@ -986,6 +992,7 @@ int dng_scan_open(const dng_plan *plan, int device, dng_scan **out, char *err,
 		if (const char *ev = getenv("DNG_F_WARPS")) {
 			s->f_nt = atoi(ev) >= 28 ? DNG_F_NT : 768;
 			s->f_probed = true;
+			s->f_forced = true;
 		}
 		if (getenv("DNG_FAST") && atoi(getenv("DNG_FAST")) == 0)
 			s->fplan.ok = 0;
@@ -1082,6 +1089,18 @@ int dng_scan_open(const dng_plan *plan, int device, dng_scan **out, char *err,
 			c2 <<= 1;
 		s->table_cap = c2;
 		size_t arena = env_size("DNG_ARENA_BYTES", (size_t)64 << 20);
+		if (arena > DNG_ARENA_MAX) {
+			/* key offsets and the bump offset are u32: refused, not
+			 * truncated.  The offset passes the cap only by the keys
+			 * claimed while the arena fills up (global_find: at most
+			 * one per resident thread, 520 B each, < 160 MiB on an
+			 * H100), which 2 GiB leaves room for whatever the table
+			 * size */
+			rc = s->fail(DNG_EINVAL, "DNG_ARENA_BYTES " +
+			    std::to_string(arena) + " is larger than the key arena "
+			    "can address (" + std::to_string(DNG_ARENA_MAX) + ")");
+			break;
+		}
 		if ((rc = s->cuda(DEV_ALLOC(s, &s->tab.entries,
 		    c2 * sizeof (GEntry)), "cudaMalloc table")))
 			break;
@@ -1758,6 +1777,23 @@ int dng_scan_kernel_stats(dng_scan *s, double *kernel_ms, uint64_t *launches,
 		*launches = s->launches;
 	if (kernel_bytes)
 		*kernel_bytes = s->kernel_bytes;
+	return DNG_OK;
+}
+
+int dng_scan_tally_stats(dng_scan *s, uint64_t *inline_overflow, int *f_warps)
+{
+	if (!s)
+		return DNG_EINVAL;
+	cudaSetDevice(s->device);
+	if (dng_scan_sync(s))
+		return s->err_code;
+	unsigned long long c = 0;
+	CK(s, cudaMemcpy(&c, s->d_counters + CTR_OVER, sizeof (c),
+	    cudaMemcpyDeviceToHost));
+	if (inline_overflow)
+		*inline_overflow = c;
+	if (f_warps)
+		*f_warps = (int)(s->f_nt / 32);
 	return DNG_OK;
 }
 

@@ -160,7 +160,12 @@ __device__ __forceinline__ u32 global_find(const GTable &t, u64 h,
 			unsigned long long old = atomicCAS(&e->tag, 0ull, claim);
 			if (old == 0) {
 				u32 need = (klen + 7) & ~7u;
-				u32 off = atomicAdd(&t.misc[0], need);
+				/* once the arena is full the offset stops growing
+				 * (only keys claimed at that moment push it past
+				 * the cap), so it cannot wrap around 2^32 */
+				u32 off = *(volatile u32 *)&t.misc[0];
+				if (off + need <= t.arena_cap)
+					off = atomicAdd(&t.misc[0], need);
 				if (off + need > t.arena_cap) {
 					atomicOr(&t.misc[2], ST_ARENA_FULL);
 					off = 0;
@@ -726,7 +731,9 @@ __device__ __forceinline__ void flush_tally(const STab &stab, u32 s1slots,
 	__syncthreads();
 	for (u32 i = tid; i < s1slots; i += blockDim.x) {
 		const SSlot1 *s = &stab.s1[i];
-		if (s->tag != 0 && s->count)
+		/* (a count of 0 is a key all of whose points weighed 0: it is
+		 * still a point of the result, with value 0) */
+		if (s->tag != 0)
 			global_add(tab, key_hash_words(s->key, s->klen),
 			    (const u8 *)s->key, s->klen,
 			    (unsigned long long)s->count);

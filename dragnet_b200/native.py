@@ -73,6 +73,8 @@ _SIGS = [
     ('dng_scan_kernel_stats', ctypes.c_int,
      [_P, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_uint64),
       ctypes.POINTER(ctypes.c_uint64)]),
+    ('dng_scan_tally_stats', ctypes.c_int,
+     [_P, ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_int)]),
     ('dng_scan_set_templates', ctypes.c_int, [_P, ctypes.c_int]),
     ('dng_scan_template_stats', ctypes.c_int,
      [_P, ctypes.POINTER(ctypes.c_uint64), ctypes.POINTER(ctypes.c_uint64)]),
@@ -349,9 +351,14 @@ class Scan(object):
         _check(lib().dng_scan_kernel_stats(self.handle, ctypes.byref(ms),
                                            ctypes.byref(n), ctypes.byref(b)),
                self.handle)
+        over = ctypes.c_uint64()
+        fw = ctypes.c_int()
+        _check(lib().dng_scan_tally_stats(self.handle, ctypes.byref(over),
+                                          ctypes.byref(fw)), self.handle)
         return {'kernel_ms': ms.value, 'launches': int(n.value),
                 'kernel_bytes': int(b.value),
-                'all_launches': int(lib().dng_scan_launch_count(self.handle))}
+                'all_launches': int(lib().dng_scan_launch_count(self.handle)),
+                'inline_overflow': int(over.value), 'f_warps': int(fw.value)}
 
     def set_templates(self, enable):
         """Record templates on/off (default on); before the first feed."""

@@ -148,6 +148,14 @@ void dng_release_cached(void);
  * the number of kernel launches since open; for bench.py's roofline. */
 int dng_scan_kernel_stats(dng_scan *scan, double *kernel_ms,
     uint64_t *launches, uint64_t *kernel_bytes);
+/*
+ * The F kernel's tally cache: *inline_overflow = records whose key its inline
+ * tier had no slot for (they took the general tally path), *f_warps = warps
+ * per CTA it launches with now (28 or 24; the scan drops to 24 when keys
+ * overflow, environment DNG_F_WARPS=28|24 sets the start).  Read-only.
+ */
+int dng_scan_tally_stats(dng_scan *scan, uint64_t *inline_overflow,
+    int *f_warps);
 
 /*
  * Record templates: the scan learns the few shapes (key order + punctuation)

@@ -303,3 +303,331 @@ def template_fuzz_lines(seed, n, nshapes=6):
             text = text.replace(':', ' :', 1)
         out.append(text.encode('utf-8'))
     return out
+
+
+# ---------------------------------------------------------------------------
+# group-by corpora (tests/test_aggregation_host.py, test_gpu_aggregation.py):
+# many distinct keys, keys whose hashes collide on purpose, key lengths at the
+# tally tiers' edges, weights.  Everything is a function of its arguments.
+# ---------------------------------------------------------------------------
+
+M64 = (1 << 64) - 1
+M32 = (1 << 32) - 1
+KEY_MAX = 512           # plan.h: longest encoded group key
+SKEY = 40               # scan_kernel.cuh DNG_SKEY: key bytes inline in tier 1
+F_MAXKEY = 256          # fast.h: longest key the F path tallies itself
+# printable ASCII that needs no escape in a JSON string
+_PLAIN = bytes(c for c in range(0x20, 0x7f) if c not in b'"\\')
+_PLAIN_SET = frozenset(_PLAIN)
+
+
+def encode_key(*cols):
+    """The encoded group key of discrete columns (DESIGN §2): per column a
+    little-endian u16 length, then the bytes of String(value)."""
+    return b''.join(len(c).to_bytes(2, 'little') + c for c in cols)
+
+
+def _g_step(h, w):
+    h ^= w
+    h = (h * 0xff51afd7ed558ccd) & M64
+    return h ^ (h >> 32)
+
+
+def _g_words(key):
+    key = key + b'\0' * (-len(key) % 8)
+    return [int.from_bytes(key[i:i + 8], 'little')
+            for i in range(0, len(key), 8)]
+
+
+def key_hash(key):
+    """record.cuh key_hash: the general kernels' 64-bit hash of a key."""
+    h = 0x9E3779B97F4A7C15 ^ ((len(key) * 0xff51afd7ed558ccd) & M64)
+    for w in _g_words(key):
+        h = _g_step(h, w)
+    h ^= h >> 29
+    h = (h * 0xc4ceb9fe1a85ec53) & M64
+    return h ^ (h >> 32)
+
+
+def _fmix(h, w):
+    h = ((h ^ w) * 0x9E3779B1) & M32
+    return h ^ (h >> 15)
+
+
+def _f_state(s, nwords=None):
+    """fast.cuh fkey_hash of one discrete column s, before its finaliser,
+    after the first nwords 4-byte words of s (all of them by default)."""
+    h = _fmix(0x2545F491, len(s))
+    p = s + b'\0' * (-len(s) % 4)
+    words = [int.from_bytes(p[i:i + 4], 'little') for i in range(0, len(p), 4)]
+    for w in words[:nwords]:
+        h = _fmix(h, w)
+    return h
+
+
+def fkey_hash(s):
+    """fast.cuh fkey_hash of a plan with one discrete column, value s."""
+    h = _f_state(s)
+    h ^= h >> 16
+    h = (h * 0x85ebca6b) & M32
+    return h ^ (h >> 13)
+
+
+def _rand_plain(rng, n):
+    return bytes(rng.choice(_PLAIN) for _ in range(n))
+
+
+def g_collisions(slen, count, seed):
+    """count strings of slen bytes (slen + 2 a multiple of 8, >= 22) whose
+    one-column keys have the same 64-bit general hash: equal first word, the
+    second-to-last word drawn at random, the last one solved for (the hash
+    is invertible word by word) until it is printable."""
+    klen = slen + 2
+    assert klen % 8 == 0 and klen >= 24
+    rng = random.Random(seed)
+    base = _rand_plain(rng, slen)
+    key = encode_key(base)
+    words = _g_words(key)
+    h = 0x9E3779B97F4A7C15 ^ ((klen * 0xff51afd7ed558ccd) & M64)
+    for w in words[:-2]:
+        h = _g_step(h, w)
+    target = _g_step(h, words[-2]) ^ words[-1]
+    out = {base}
+    while len(out) < count:
+        w1 = _rand_plain(rng, 8)
+        w2 = (target ^ _g_step(h, int.from_bytes(w1, 'little'))).to_bytes(
+            8, 'little')
+        if _PLAIN_SET.issuperset(w2):
+            out.add(base[:slen - 16] + w1 + w2)
+    out = sorted(out)
+    assert len({key_hash(encode_key(s)) for s in out}) == 1
+    return out
+
+
+def f_collisions(slen, count, seed):
+    """count strings of slen bytes (a multiple of 4, >= 8) with the same F
+    hash (fkey_hash, one discrete column): the last word solved for."""
+    assert slen % 4 == 0 and slen >= 8
+    rng = random.Random(seed)
+    base = _rand_plain(rng, slen)
+    nw = slen // 4
+    h = _f_state(base, nw - 2)
+    target = _f_state(base)
+    out = {base}
+    while len(out) < count:
+        w1 = _rand_plain(rng, 4)
+        hs = _fmix(h, int.from_bytes(w1, 'little'))
+        # _fmix(hs, w) == target  <=>  (hs ^ w) * K == unmix(target)
+        x = target
+        x ^= x >> 15
+        x ^= x >> 30
+        x = (x * pow(0x9E3779B1, -1, 1 << 32)) & M32
+        w2 = (x ^ hs).to_bytes(4, 'little')
+        if _PLAIN_SET.issuperset(w2):
+            out.add(base[:slen - 8] + w1 + w2)
+    out = sorted(out)
+    assert len({fkey_hash(s) for s in out}) == 1
+    return out
+
+
+GLOBAL_SLOT = 1020
+
+
+def index_collisions(slen, count, hashfn, shift, bits, seed, pool=60000,
+                     slot=None):
+    """count distinct strings of slen bytes whose hashfn(string) agree in
+    bits [shift, shift + bits) (they probe from the same slot of a table of
+    up to 2^bits entries) but not in the whole hash: the largest such group
+    of a seeded pool, or the group of that slot."""
+    rng = random.Random(seed)
+    groups = {}
+    mask = (1 << bits) - 1
+    for _ in range(pool):
+        s = _rand_plain(rng, slen)
+        groups.setdefault((hashfn(s) >> shift) & mask, set()).add(s)
+    best = max(groups.values(), key=len) if slot is None else groups[slot]
+    assert len(best) >= count, (len(best), count)
+    return sorted(best)[:count]
+
+
+def gkey_hash(s):
+    return key_hash(encode_key(s))
+
+
+def collision_groups(seed=0):
+    """name -> strings that meet in one slot of one tally tier (see
+    test_aggregation_host.py for what each one has to reach)."""
+    return {
+        # F inline tier: index (h >> 7) & mask1, mask1 <= 1023, 8 probes
+        'f_index': index_collisions(28, 40, fkey_hash, 7, 10, seed + 1),
+        # F inline tier: equal claims, fkey_equal decides
+        'f_full': f_collisions(24, 40, seed + 2),
+        # general tier 1 (keys <= 40 B): bits 40-49, 8 probes
+        'g1_index': index_collisions(30, 40, gkey_hash, 40, 10, seed + 3),
+        # general tier 1, equal tags: the inline word compare decides
+        'g1_full': g_collisions(22, 40, seed + 4),
+        # general tier 2 (keys > 40 B): bits 28-39, 24 probes
+        'g2_index': index_collisions(46, 40, gkey_hash, 28, 12, seed + 5,
+                                     pool=160000),
+        # tier 2 and the global table, equal tags: the arena bytes decide
+        'g2_full': g_collisions(46, 40, seed + 6),
+        # global table of DNG_TABLE_CAP=1024: bits 17-26
+        # global table of DNG_TABLE_CAP=1024: bits 17-26, home slot 1020,
+        # so that the chain wraps around the table's end
+        'global_index': index_collisions(20, 40, gkey_hash, 17, 10,
+                                         seed + 7, slot=GLOBAL_SLOT),
+    }
+
+
+def kv_line(key, v, pad):
+    return b'{"key":' + json.dumps(key.decode('latin-1')).encode() + \
+        b',"val":%d,"pad":"%s"}' % (v, pad)
+
+
+def kv_lines(keys, n, seed, pad=40):
+    """n records {"key":key,"val":..,"pad":..} cycling through keys in a seeded
+    order, so that every chunk (and CTA) sees keys of every group."""
+    rng = random.Random(seed)
+    padb = b'p' * pad
+    order = list(keys)
+    out = []
+    while len(out) < n:
+        rng.shuffle(order)
+        out.extend(kv_line(k, i % 7, padb) for i, k in
+                   enumerate(order[:n - len(out)]))
+    return out
+
+
+def sweep_lines(k, n, seed=0):
+    """n records over k distinct keys k%d (lengths 2-8: tier 1 everywhere)."""
+    rng = random.Random(seed)
+    return [b'{"key":"k%d","val":%d,"pad":"%s"}' %
+            (rng.randrange(k), i % 7, b'p' * (30 + i % 11)) for i in range(n)]
+
+
+def skew_lines(n, seed=0, hot=16, tail=100000):
+    """Half the records on hot keys, the rest over a long tail: the hot keys
+    are in every CTA's tier 1 while the tail fills tier 2 and the table."""
+    rng = random.Random(seed)
+    out = []
+    for i in range(n):
+        key = b'hot%d' % rng.randrange(hot) if i % 2 else \
+            b'tail-%d' % rng.randrange(tail)
+        out.append(b'{"key":"%s","val":%d,"pad":"%s"}' % (key, i % 5,
+                                                      b'q' * (24 + i % 13)))
+    return out
+
+
+# encoded key lengths (one column: 2 + len): both sides of the inline tier
+# (40), of 8-byte word edges, of the F path's 256 and of KEY_MAX (512; the
+# longest accepted one-column key is 512 bytes: a 510-byte string)
+KEY_LENGTHS = [38, 39, 40, 41, 42, 47, 48, 49, 254, 255, 256, 257, 258, 511,
+               512]
+
+
+def key_length_lines(two=False, seed=0, reps=40):
+    """Records whose keys (-b key, or with two=True -b key,key2) are KEY_LENGTHS
+    long, a few variants of each, repeated so that every key is tallied from
+    many CTAs."""
+    rng = random.Random(seed)
+    recs = []
+    for kl in KEY_LENGTHS:
+        for var in range(4):
+            s = (b'%d-%d-' % (kl, var) + _rand_plain(rng, kl))[:kl - 2]
+            if not two:
+                recs.append(b'{"key":"%s","pad":"x"}' % s)
+                continue
+            # two columns: 2 + a + 2 + b == kl, a <= 500
+            a = min(len(s) - 2, 500) if var % 2 else (len(s) - 2) // 2
+            recs.append(b'{"key":"%s","key2":"%s","pad":"y"}' % (s[:a],
+                                                             s[a:len(s) - 2]))
+    out = []
+    for r in range(reps):
+        rng.shuffle(recs)
+        out.extend(recs)
+    return out
+
+
+def merge_apart_lines(reps=50):
+    """Keys that must stay apart although their bytes nearly agree, and
+    spellings of one value that must merge into one key."""
+    apart = []
+    for n in (5, 6, 7, 13, 14, 15, 21, 22, 23, 37, 38, 39, 45, 46, 47):
+        stem = b'w' * (n - 1)
+        # differ only in the last byte (the last, zero padded key word)
+        apart += [stem + b'a', stem + b'b', stem + b'\x7e']
+    recs = [b'{"key":"%s","key2":"z","pad":"mmmmmmmm"}' % s for s in apart]
+    recs += [
+        b'{"key":"a","key2":"z","pad":"mmmmmmmm"}',
+        b'{"key":"a\\u0000","key2":"z","pad":"mmmmmmmm"}',
+        b'{"key":"xy","key2":"","pad":"mmmmmmmm"}',
+        b'{"key":"x","key2":"y","pad":"mmmmmmmm"}',
+        b'{"key":"","key2":"xy","pad":"mmmmmmmm"}',
+        b'{"key":"ab","key2":"","pad":"mmmmmmmm"}',
+        b'{"key":"a","key2":"\\u0000","pad":"mmmmmmmm"}',
+        # String(value) of numbers: one key
+        b'{"key":1,"key2":"z","pad":"mmmmmmmm"}',
+        b'{"key":1.0,"key2":"z","pad":"mmmmmmmm"}',
+        b'{"key":1e0,"key2":"z","pad":"mmmmmmmm"}',
+        b'{"key":"1","key2":"z","pad":"mmmmmmmm"}',
+        b'{"key":10e-1,"key2":"z","pad":"mmmmmmmm"}',
+        b'{"key":1,"key2":1.0,"pad":"mmmmmmmm"}',
+        b'{"key":"1","key2":"1","pad":"mmmmmmmm"}',
+    ]
+    out = []
+    for r in range(reps):
+        out.extend(recs[r % len(recs):] + recs[:r % len(recs)])
+    return out
+
+
+# bucketized merges (-0 and 0, spellings of one number)
+BUCKET_LINES = [b'{"num":%s,"pad":"mmmmmmmmmmmm"}' % v for v in
+                (b'0', b'-0', b'0.0', b'-0.0', b'0e5', b'1', b'1.0', b'1e0',
+                 b'"1"', b'2', b'3', b'-1', b'255', b'256')] * 30
+
+
+# json-skinner weights: the tally's w <= 255 inline route and w > 255 route
+WEIGHTS = [b'0', b'1', b'254', b'255', b'256', b'257', b'2147483648',
+           b'4294967295', b'4294967296', b'1099511627776', b'9007199254740992',
+           b'2.5e2', b'256.0', b'9007199254740993', b'9007199254740994']
+
+
+def weight_lines(seed=0, nkeys=20000, n=200000):
+    """Skinner points: every weight on three shared keys (each key takes the
+    whole list in turn; the weights of 2^40 and more only in the first eight
+    rounds per key), weights <= 255 and > 255 mixed over a high-cardinality
+    set, and keys all of whose points weigh 0.  Every sum stays below 2^63
+    (weight_sums)."""
+    rng = random.Random(seed)
+    nw = len(WEIGHTS)
+    out = []
+    for i in range(n):
+        if i % 4 == 0:
+            j = i // 4
+            k = b'shared%d' % (j // nw % 3)
+            w = WEIGHTS[j % nw] if j < nw * 3 * 8 else WEIGHTS[j % 8]
+        elif i % 50 == 1:
+            # keys all of whose points weigh 0: points of value 0
+            k = b'zero%d' % (i % 7)
+            w = rng.choice([b'0', b'0.0', b'-0'])
+        else:
+            k = b'key%d' % rng.randrange(nkeys)
+            w = rng.choice(WEIGHTS[:11] + [b'2.5e2', b'256.0'])
+        out.append(b'{"fields":{"key":"%s"},"value":%s}' % (k, w))
+    return out
+
+
+def weight_sums(lines):
+    """key -> exact sum of the weight_lines records' values, as Python
+    integers: a value counts when it is a whole number from 0 to 2^53 as a
+    double (9007199254740993 reads as 2^53; 9007199254740994 does not
+    count)."""
+    sums = {}
+    for ln in lines:
+        doc = json.loads(ln)
+        v = float(doc['value'])
+        if v != int(v) or not 0 <= v <= 1 << 53:
+            continue
+        k = doc['fields']['key'].encode()
+        sums[k] = sums.get(k, 0) + int(v)
+    return sums

@@ -210,6 +210,28 @@ int main(int argc, char **argv)
 		jm = host_jit(fblob, &FP, &jmem);
 		*jmem = jbuf;
 	}
+	/* DNG_HOSTCHECK_KEYS=PATH: one line per tallied record, "KEY FHASH GHASH"
+	 * (key bytes in hex; the F path's 32-bit hash, "-" when the F path did
+	 * not take the record; the general 64-bit hash), so that tests can pick
+	 * keys that collide in the device's tally tables.  Skips the all-pairs
+	 * fkey_equal check, which is quadratic in the keys. */
+	FILE *keys_out = nullptr;
+	if (const char *kp = getenv("DNG_HOSTCHECK_KEYS")) {
+		keys_out = fopen(kp, "w");
+		if (!keys_out) {
+			fprintf(stderr, "cannot write %s\n", kp);
+			return 2;
+		}
+	}
+	auto dump_key = [&](const u8 *k, u32 klen, const char *fh) {
+		static u8 padded[KEY_MAX + 64];
+		memset(padded, 0, sizeof (padded));
+		memcpy(padded, k, klen);
+		for (u32 i = 0; i < klen; i++)
+			fprintf(keys_out, "%02x", k[i]);
+		fprintf(keys_out, " %s %016llx\n", fh,
+		    (unsigned long long)key_hash(padded, klen));
+	};
 	static LocalCounters MCs[MAX_METRICS];
 	memset(MCs, 0, sizeof (MCs));
 	std::map<std::string, uint64_t> table;
@@ -283,7 +305,14 @@ int main(int argc, char **argv)
 						fprintf(stderr, "fkey_hash: unstable\n");
 						return 3;
 					}
+					if (keys_out) {
+						char fh[16];
+						snprintf(fh, sizeof (fh), "%08x", h);
+						dump_key(kbuf, klen, fh);
+					}
 					for (auto &kv : fhashes) {
+						if (keys_out)
+							break;
 						if (kv.first == key ||
 						    kv.first.size() != key.size())
 							continue;
@@ -353,6 +382,8 @@ int main(int argc, char **argv)
 					LocalCounters &MC = mi ? MCs[mi] : C;
 					if (process_metric(rec, plan.dev, mi, R, MC,
 					    kbuf, klen)) {
+						if (keys_out)
+							dump_key(kbuf, klen, "-");
 						table[std::string((char *)kbuf,
 						    klen)] += w;
 					}
@@ -361,6 +392,8 @@ int main(int argc, char **argv)
 		}
 		pos = end + 1;
 	}
+	if (keys_out)
+		fclose(keys_out);
 	dng_result res;
 	res.init_from_plan(&plan);
 	for (auto &kv : table) {
