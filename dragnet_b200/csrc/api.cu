@@ -179,17 +179,11 @@ struct dng_scan {
 	bool finished = false;
 	/* record templates (tmpl.h), learned from the head of the input */
 	bool tmpl_enabled = true, tmpl_tried = false;
-	/* kernel geometry: per-warp chunks for short lines, CTA tiles otherwise */
-	bool warp_kernel = false;
-	u32 wslice = DNG_W_SLICE_MAX;	/* bytes per lane of a warp's chunk */
-	int kernel_pref = 0;		/* DNG_KERNEL: 0 auto, 1 tile, 2 warp, 3 fast */
+	KernelChoice kc;		/* which kernel, at what geometry */
 	u32 w_sslots = 0, w_s1slots = 0;
 	/* counters of finished launches, copied to pinned memory after every
 	 * launch: lets the host notice that the input changed character */
 	unsigned long long *h_live = nullptr;
-	unsigned long long learn_lines = 0, learn_tmpl = 0;
-	unsigned long long seen_lines = 0, seen_long = 0;
-	int relearns = 0;
 	u8 *d_tmpl = nullptr;
 	u32 tmpl_bytes = 0, ntemplates = 0;
 	/* the F path (fast.h): its plan, its templates, its miss list */
@@ -197,14 +191,6 @@ struct dng_scan {
 	FPlan *d_fplan = nullptr;
 	u8 *d_ftmpl = nullptr;
 	u32 ftmpl_bytes = 0, nftemplates = 0, ftmpl_leaf_off = 0, ftmpl_pool_off = 0;
-	bool f_kernel = false;
-	u32 f_nt = DNG_F_NT;		/* threads of its CTA: DNG_F_NT, or 768 when
-					 * the tally cache needs the shared memory */
-	unsigned long long seen_over = 0, seen_aggr = 0;
-	bool f_probed = false;
-	bool f_forced = false;		/* DNG_F_WARPS chose f_nt: not remembered */
-	u32 f_nsl = 13;			/* 16-byte units per lane slice */
-	double mean_line = 224;		/* of the sample the templates came from */
 	u32 f_smem_max = 0;		/* dynamic shared memory a CTA may ask for */
 	/* run-time compiled matcher (jit.h): 0 off, 1 in the background, 2 wait */
 	int jit_mode = 1;
@@ -268,43 +254,17 @@ __global__ void resolve_pairs_kernel(const DevPlan *plan, const u8 *lines,
 
 /*
  * The F path's templates (fast.h): the same candidates, their captures indexed
- * by path, compact literals.  The F kernel is chosen when they cover the
- * sample (results never depend on that choice, only the speed does).
+ * by path, compact literals.  `blob` keeps them for the compiled matcher, `t`
+ * says what they cover of the sample.
  */
-/*
- * What a scan of this plan found out about its tally cache (f_nt), kept for
- * the scans of the same plan that follow in this process: they start with it
- * and need no probe launch.
- */
-static std::mutex g_fnt_mu;
-static std::map<unsigned long long, u32> g_fnt_memo;
-
-static unsigned long long fplan_hash(const FPlan &F)
-{
-	unsigned long long h = 1469598103934665603ull;
-	const u8 *p = (const u8 *)&F;
-	for (size_t i = 0; i < sizeof (F); i++)
-		h = (h ^ p[i]) * 1099511628211ull;
-	return h;
-}
-
-static void fnt_remember(const dng_scan *s)
-{
-	/* a count forced by DNG_F_WARPS says nothing about the plan, and would
-	 * otherwise stay in force for every later scan of it in this process */
-	if (s->f_forced)
-		return;
-	std::lock_guard<std::mutex> g(g_fnt_mu);
-	g_fnt_memo[fplan_hash(s->fplan)] = s->f_nt;
-}
-
 int learn_ftemplates(dng_scan *s, const std::vector<TCandidate> &cands,
-    const std::vector<TResolved> &res, size_t sampled_lines)
+    const std::vector<TResolved> &res, size_t sampled_lines,
+    std::vector<u8> &blob, KcTemplates &t)
 {
 	std::vector<TResolved> fres(res.size());
 	for (size_t i = 0; i < res.size(); i++)
 		fplan_resolve(s->plan.dev, res[i], fres[i]);
-	std::vector<u8> blob, accepted;
+	std::vector<u8> accepted;
 	u32 nt = 0;
 	tmpl_build(cands, fres, TMPL_RESERVE, blob, &nt, true, &accepted);
 	cached_free(s->d_ftmpl);
@@ -316,10 +276,12 @@ int learn_ftemplates(dng_scan *s, const std::vector<TCandidate> &cands,
 		s->ftmpl_leaf_off = th->leaf_off;
 		s->ftmpl_pool_off = th->pool_off;
 	}
-	size_t covered = 0;
+	t.learned = true;
+	t.blob = !blob.empty();
+	t.lines = sampled_lines;
 	for (size_t i = 0; i < cands.size(); i++)
 		if (accepted[i])
-			covered += cands[i].count;
+			t.covered += cands[i].count;
 	if (!blob.empty()) {
 		size_t padded = (blob.size() + 127) & ~(size_t)127;
 		blob.resize(padded, 0);
@@ -330,96 +292,21 @@ int learn_ftemplates(dng_scan *s, const std::vector<TCandidate> &cands,
 		s->ftmpl_bytes = (u32)padded;
 		s->nftemplates = nt;
 	}
-	s->jit.reset();
-	if (s->jit_mode && !blob.empty())
-		s->jit = jit_request(jit_source(blob.data(), blob.size(), &s->fplan),
-		    (int)s->f_nsl, s->device, (int)s->f_smem_max,
-		    s->jit_mode == 2);
-	if (s->kernel_pref == 0)
-		s->f_kernel = s->warp_kernel && !blob.empty() &&
-		    covered * 10 >= sampled_lines * 9 &&
-		    s->mean_line * DNG_F_NLCAP >= 32.0 * 16 * s->f_nsl * 1.5;
 	return 0;
 }
 
 /*
- * Learn record templates from the head of the first data this scan sees
- * (device memory): skeletons on the host (lexical only), what their
- * wildcards mean to the plan from the device's own parser.  Failure to learn
- * anything is not an error: the kernel then parses every record itself.
+ * Record templates from a sample (host memory): skeletons on the host
+ * (lexical only), what their wildcards mean to the plan from the device's own
+ * parser.  Failure to learn anything is not an error: the kernel then parses
+ * every record itself.
  */
-int learn_templates(dng_scan *s, const u8 *data, unsigned long long start,
-    unsigned long long nbytes)
+int build_templates(dng_scan *s, const u8 *head, size_t n,
+    std::vector<u8> &fblob, KcTemplates &ft)
 {
-	s->tmpl_tried = true;
-	if (!s->tmpl_enabled && s->kernel_pref != 0)
-		return 0;
-	size_t n = (size_t)std::min<unsigned long long>(nbytes - start,
-	    TMPL_SAMPLE_BYTES);
-	/* pinned (and cached) so that the copy is a plain DMA */
-	u8 *hbuf = nullptr;
-	CK(s, HOST_ALLOC(&hbuf, TMPL_SAMPLE_BYTES));
-	struct Release {
-		u8 *p;
-		~Release() { cached_free(p); }
-	} release{hbuf};
-	CK(s, cudaMemcpyAsync(hbuf, data + start, n, cudaMemcpyDeviceToHost,
-	    s->stream));
-	CK(s, cudaStreamSynchronize(s->stream));
-	struct { u8 *p; u8 *data() const { return p; }
-	    u8 operator[](size_t i) const { return p[i]; } } head{hbuf};
-	if (s->kernel_pref == 0) {
-		/* short lines: every warp stages its own chunk (scan_kernel_w);
-		 * otherwise CTA-wide tiles, whose window holds long lines */
-		size_t longest = 0, run = 0;
-		for (size_t i = 0; i < n; i++) {
-			if (head[i] == '\n') {
-				longest = std::max(longest, run);
-				run = 0;
-			} else {
-				run++;
-			}
-		}
-		longest = std::max(longest, run);
-		s->warp_kernel = longest <= DNG_W_MAXLINE;
-	}
-	{
-		/* chunk size: the lane slice (16 x odd bytes) whose chunk holds
-		 * the most records per 32-lane pass, given the mean line */
-		size_t nl = 0;
-		for (size_t i = 0; i < n; i++)
-			nl += head[i] == '\n';
-		double mean = nl ? (double)n / (double)nl : 224.0;
-		s->mean_line = mean;
-		double best = -1;
-		for (u32 sl = 112; sl <= DNG_W_SLICE_MAX; sl += 32) {
-			double recs = 32.0 * sl / mean;
-			double passes = ceil((recs + 1.5) / 32.0);
-			double util = recs / (32.0 * passes);
-			if (util >= best) {
-				best = util;
-				s->wslice = sl;
-			}
-		}
-		/* the F kernel indexes at most DNG_F_NLCAP lines per chunk:
-		 * the largest such slice with the best lane use */
-		best = -1;
-		s->f_nsl = 7;
-		for (u32 sl = 112; sl <= DNG_W_SLICE_MAX; sl += 32) {
-			double recs = 32.0 * sl / mean;
-			double passes = ceil((recs + 1.5) / 32.0);
-			double util = recs / (32.0 * passes);
-			if (recs * 1.25 <= DNG_F_NLCAP && util >= best) {
-				best = util;
-				s->f_nsl = sl / 16;
-			}
-		}
-	}
-	if (!s->tmpl_enabled)
-		return 0;
 	std::vector<TCandidate> cands;
 	size_t sampled_lines = 0;
-	tmpl_candidates(head.data(), n, TMPL_MAX_LEAVES, cands, &sampled_lines);
+	tmpl_candidates(head, n, TMPL_MAX_LEAVES, cands, &sampled_lines);
 	if (cands.empty())
 		return 0;
 	std::vector<u8> lines;
@@ -469,7 +356,8 @@ int learn_templates(dng_scan *s, const u8 *data, unsigned long long start,
 	cached_free(d_res);
 	if (e != cudaSuccess)
 		return s->cuda(e, "template resolve");
-	if (s->fplan.ok && learn_ftemplates(s, cands, res, sampled_lines))
+	if (s->kc.f_ok && learn_ftemplates(s, cands, res, sampled_lines, fblob,
+	    ft))
 		return s->err_code;
 	std::vector<u8> blob;
 	u32 nt = 0;
@@ -491,30 +379,89 @@ int learn_templates(dng_scan *s, const u8 *data, unsigned long long start,
 	return 0;
 }
 
-template <int NSL>
-void launch_fkernel(dng_scan *s, const FScanArgs &a, u32 grid)
+/*
+ * Sample the head of data[start, nbytes) (device memory): its lines set the
+ * kernel geometry, its records the templates.
+ */
+int learn_templates(dng_scan *s, const u8 *data, unsigned long long start,
+    unsigned long long nbytes)
 {
-	scan_kernel_f<NSL><<<grid, s->f_nt, fkernel_smem<NSL>(a.tmpl_bytes,
-	    a.s1slots, a.sslots, a.nrows, s->f_nt / 32), s->stream>>>(a);
+	s->tmpl_tried = true;
+	if (!kc_wants_sample(s->kc, s->tmpl_enabled))
+		return 0;
+	size_t n = (size_t)std::min<unsigned long long>(nbytes - start,
+	    TMPL_SAMPLE_BYTES);
+	/* pinned (and cached) so that the copy is a plain DMA */
+	u8 *hbuf = nullptr;
+	CK(s, HOST_ALLOC(&hbuf, TMPL_SAMPLE_BYTES));
+	struct Release {
+		u8 *p;
+		~Release() { cached_free(p); }
+	} release{hbuf};
+	CK(s, cudaMemcpyAsync(hbuf, data + start, n, cudaMemcpyDeviceToHost,
+	    s->stream));
+	CK(s, cudaStreamSynchronize(s->stream));
+	std::vector<u8> fblob;
+	KcTemplates ft;
+	if (s->tmpl_enabled && build_templates(s, hbuf, n, fblob, ft))
+		return s->err_code;
+	kc_sample(s->kc, hbuf, n, ft);
+	if (ft.learned) {
+		s->jit.reset();
+		if (s->jit_mode && !fblob.empty())
+			s->jit = jit_request(jit_source(fblob.data(), fblob.size(),
+			    &s->fplan), (int)s->kc.f_nsl, s->device,
+			    (int)s->f_smem_max, s->jit_mode == 2);
+	}
+	return 0;
 }
 
-/* tally-cache sizes of the F kernel: what its buffers leave */
-template <int NSL>
-void fkernel_slots(const dng_scan *s, u32 nrows, u32 tmpl_room, u32 *s1, u32 *s2)
+/* tier 2 of a tally cache: as many compact slots as fit in `room` (a power of
+ * two) */
+u32 tier2_slots(size_t room)
 {
-	const size_t fixed = fkernel_smem<NSL>(tmpl_room, 0, 0, nrows,
-	    s->f_nt / 32);
-	const size_t room = s->f_smem_max > fixed ? s->f_smem_max - fixed : 0;
-	u32 n1 = 32;
-	while (n1 < 1024 && (size_t)n1 * 2 * sizeof (SSlot1) +
-	    DNG_SSLOTS_MIN * sizeof (SSlot) <= room * 3 / 4)
-		n1 *= 2;
-	const size_t left = room - std::min(room, (size_t)n1 * sizeof (SSlot1));
-	u32 n2 = DNG_SSLOTS_MIN;
-	while (n2 * 2 <= DNG_SSLOTS_MAX && (size_t)n2 * 2 * sizeof (SSlot) <= left)
-		n2 *= 2;
-	*s1 = n1;
-	*s2 = n2;
+	u32 n = DNG_SSLOTS_MIN;
+	while (n * 2 <= DNG_SSLOTS_MAX && (size_t)n * 2 * sizeof (SSlot) <= room)
+		n *= 2;
+	return n;
+}
+
+/* the F kernel for lane slices of nsl x 16 bytes, and its per-warp shared
+ * memory */
+const void *fkernel(u32 nsl, u32 *warp_bytes)
+{
+	switch (nsl) {
+	case 7:
+		*warp_bytes = FWarpSmem<7>::BYTES;
+		return (const void *)scan_kernel_f<7>;
+	case 9:
+		*warp_bytes = FWarpSmem<9>::BYTES;
+		return (const void *)scan_kernel_f<9>;
+	case 11:
+		*warp_bytes = FWarpSmem<11>::BYTES;
+		return (const void *)scan_kernel_f<11>;
+	default:
+		*warp_bytes = FWarpSmem<13>::BYTES;
+		return (const void *)scan_kernel_f<13>;
+	}
+}
+
+/* after a scan launch: its timing, the pinned copy of the counters the next
+ * launch decides on, the counts */
+void launched(dng_scan *s, cudaEvent_t e0, unsigned long long bytes)
+{
+	cudaEvent_t e1 = get_event(s);
+	cudaEventRecord(e1, s->stream);
+	if (!s->h_live && HOST_ALLOC(&s->h_live, NCTR * sizeof (unsigned long long))
+	    == cudaSuccess)
+		memset(s->h_live, 0, NCTR * sizeof (unsigned long long));
+	if (s->h_live)
+		cudaMemcpyAsync(s->h_live, s->d_counters,
+		    NCTR * sizeof (unsigned long long), cudaMemcpyDeviceToHost,
+		    s->stream);
+	s->ev_pairs.emplace_back(e0, e1);
+	s->launches++;
+	s->kernel_bytes += bytes;
 }
 
 /*
@@ -553,10 +500,10 @@ int launch_fscan(dng_scan *s, const u8 *data, unsigned long long start,
 	a.miss = s->d_miss;
 	a.miss_cap = s->miss_cap;
 	a.miss_n = s->d_miss_n;
-	const u32 nsl = s->f_nsl;
+	const u32 nsl = s->kc.f_nsl;
 	const unsigned long long chunk = 32ull * 16 * nsl;
 	a.nchunks = (u32)((nbytes + chunk - 1) / chunk);
-	const u32 nw = s->f_nt / 32;
+	const u32 nw = s->kc.f_nw;
 	const u32 grid = std::min<u32>((a.nchunks + nw - 1) / nw,
 	    (u32)s->sm_count);
 	/* segments: long enough to amortise the pre-lap, short enough to keep
@@ -567,53 +514,34 @@ int launch_fscan(dng_scan *s, const u8 *data, unsigned long long start,
 	/* the segment queue: [1] of the miss counter's allocation */
 	a.seg_next = s->d_miss_n + 1;
 	cudaMemsetAsync(s->d_miss_n, 0, 2 * sizeof (u32), s->stream);
-	cudaEvent_t e0 = get_event(s), e1 = get_event(s);
+	cudaEvent_t e0 = get_event(s);
 	cudaEventRecord(e0, s->stream);
 	/* the matcher compiled for these templates, once it is there */
 	const bool jit = s->jit && s->jit->state.load() == 1 && s->ftmpl_bytes;
+	u32 warp_bytes = 0;
+	const void *kern = fkernel(nsl, &warp_bytes);
 	/* (the compiled matcher has the templates in its code: no trie in shared
 	 * memory, more of it for the tally cache) */
 	const u32 tmpl_room = jit ? 0 : (u32)TMPL_RESERVE;
-	if (jit)
-		a.tmpl_bytes = 0;
-	size_t smem = 0;
-	switch (nsl) {
-	case 7:
-		fkernel_slots<7>(s, a.nrows, tmpl_room, &a.s1slots, &a.sslots);
-		smem = fkernel_smem<7>(a.tmpl_bytes, a.s1slots, a.sslots, a.nrows,
-		    s->f_nt / 32);
-		if (!jit)
-			launch_fkernel<7>(s, a, grid);
-		break;
-	case 9:
-		fkernel_slots<9>(s, a.nrows, tmpl_room, &a.s1slots, &a.sslots);
-		smem = fkernel_smem<9>(a.tmpl_bytes, a.s1slots, a.sslots, a.nrows,
-		    s->f_nt / 32);
-		if (!jit)
-			launch_fkernel<9>(s, a, grid);
-		break;
-	case 11:
-		fkernel_slots<11>(s, a.nrows, tmpl_room, &a.s1slots, &a.sslots);
-		smem = fkernel_smem<11>(a.tmpl_bytes, a.s1slots, a.sslots, a.nrows,
-		    s->f_nt / 32);
-		if (!jit)
-			launch_fkernel<11>(s, a, grid);
-		break;
-	default:
-		fkernel_slots<13>(s, a.nrows, tmpl_room, &a.s1slots, &a.sslots);
-		smem = fkernel_smem<13>(a.tmpl_bytes, a.s1slots, a.sslots, a.nrows,
-		    s->f_nt / 32);
-		if (!jit)
-			launch_fkernel<13>(s, a, grid);
-		break;
-	}
-	cudaError_t le = cudaSuccess;
 	if (jit) {
-		void *args[] = { &a };
-		le = cudaLaunchKernel((const void *)s->jit->kern, dim3(grid),
-		    dim3(s->f_nt), args, smem, s->stream);
+		kern = (const void *)s->jit->kern;
+		a.tmpl_bytes = 0;
 		s->jit_launches++;
 	}
+	/* the tally cache takes what the buffers leave, its first tier up to
+	 * three quarters of that */
+	const size_t fixed = fkernel_smem(warp_bytes, tmpl_room, 0, 0, a.nrows, nw);
+	const size_t room = s->f_smem_max > fixed ? s->f_smem_max - fixed : 0;
+	a.s1slots = 32;
+	while (a.s1slots < 1024 && (size_t)a.s1slots * 2 * sizeof (SSlot1) +
+	    DNG_SSLOTS_MIN * sizeof (SSlot) <= room * 3 / 4)
+		a.s1slots *= 2;
+	a.sslots = tier2_slots(room - std::min(room,
+	    (size_t)a.s1slots * sizeof (SSlot1)));
+	void *args[] = { &a };
+	cudaError_t le = cudaLaunchKernel(kern, dim3(grid), dim3(32 * nw), args,
+	    fkernel_smem(warp_bytes, a.tmpl_bytes, a.s1slots, a.sslots, a.nrows,
+	    nw), s->stream);
 	if (le == cudaSuccess)
 		le = cudaGetLastError();
 	FMissArgs ma;
@@ -634,18 +562,8 @@ int launch_fscan(dng_scan *s, const u8 *data, unsigned long long start,
 		    s->stream>>>(ma);
 		le = cudaGetLastError();
 	}
-	cudaEventRecord(e1, s->stream);
-	if (!s->h_live && HOST_ALLOC(&s->h_live, NCTR * sizeof (unsigned long long))
-	    == cudaSuccess)
-		memset(s->h_live, 0, NCTR * sizeof (unsigned long long));
-	if (s->h_live)
-		cudaMemcpyAsync(s->h_live, s->d_counters,
-		    NCTR * sizeof (unsigned long long), cudaMemcpyDeviceToHost,
-		    s->stream);
-	s->ev_pairs.emplace_back(e0, e1);
-	s->launches++;
+	launched(s, e0, nbytes - start);
 	s->aux_launches++;
-	s->kernel_bytes += nbytes - start;
 	return s->cuda(le, "scan_kernel_f launch");
 }
 
@@ -659,64 +577,19 @@ int launch_scan(dng_scan *s, const u8 *data, unsigned long long start,
 		if (learn_templates(s, data, start, nbytes))
 			return s->err_code;
 	} else if (s->h_live) {
-		/*
-		 * Input that changes character mid-stream (another file,
-		 * another producer): many lines longer than a warp's pre-lap
-		 * -> the tile kernel from here on; most records missing the
-		 * templates -> learn again from this data (a few times at most;
-		 * each costs a stream synchronisation).
-		 */
 		const volatile unsigned long long *lv = s->h_live;
-		const unsigned long long lines = lv[CTR_LINES];
-		const unsigned long long nlong = lv[CTR_LONG];
-		if (lines - s->seen_lines >= 64) {
-			/* over the launches that finished since the last look */
-			if (s->warp_kernel && s->kernel_pref == 0 &&
-			    (nlong - s->seen_long) * 16 > lines - s->seen_lines)
-				s->warp_kernel = false;
-			s->seen_lines = lines;
-			s->seen_long = nlong;
-		}
-		/* keys the F kernel's inline tally tier had no room for: with 28
-		 * warps it is small; 24 leave it 30 KB more */
-		if (s->f_nt > 768 && lv[CTR_AGGR] - s->seen_aggr >= 4096) {
-			if ((lv[CTR_OVER] - s->seen_over) * 64 >
-			    lv[CTR_AGGR] - s->seen_aggr)
-				s->f_nt = 768;
-			s->seen_over = lv[CTR_OVER];
-			s->seen_aggr = lv[CTR_AGGR];
-			fnt_remember(s);
-		}
-		const unsigned long long dl = lines - s->learn_lines;
-		/* the F path only pays while it takes nearly every record: with
-		 * more than a few percent going through the miss list, learn
-		 * again; if that was already done, leave it to the general
-		 * kernels (whose second tier runs from shared memory) */
-		if (s->f_kernel && s->kernel_pref == 0 && dl > 200000 &&
-		    (dl - (lv[CTR_TMPL] - s->learn_tmpl)) * 16 > dl &&
-		    s->relearns >= 1)
-			s->f_kernel = false;
-		const bool fweak = s->f_kernel && s->kernel_pref == 0 &&
-		    (dl - (lv[CTR_TMPL] - s->learn_tmpl)) * 16 > dl;
-		if (s->tmpl_enabled && s->relearns < 3 && dl > 200000 &&
-		    ((lv[CTR_TMPL] - s->learn_tmpl) * 2 < dl || fweak)) {
-			s->relearns++;
-			const bool wk = s->warp_kernel;
+		const KcLive live = { lv[CTR_LINES], lv[CTR_LONG], lv[CTR_TMPL],
+		    lv[CTR_AGGR], lv[CTR_OVER] };
+		if (kc_counters(s->kc, live, s->tmpl_enabled)) {
 			if (learn_templates(s, data, start, nbytes))
 				return s->err_code;
-			if (!wk && s->kernel_pref == 0)
-				s->warp_kernel = false;	/* long lines were seen */
 			/* the stream is idle: the counters below are current */
-			s->learn_lines = lv[CTR_LINES];
-			s->learn_tmpl = lv[CTR_TMPL];
+			s->kc.learn_lines = lv[CTR_LINES];
+			s->kc.learn_tmpl = lv[CTR_TMPL];
 		}
 	}
-	/* (a plan with many capture rows leaves the F kernel's buffers no room) */
-	if (s->f_kernel && s->fplan.ok &&
-	    fkernel_smem<13>(TMPL_RESERVE, 32, DNG_SSLOTS_MIN, s->fplan.nrows) >
-	    s->f_smem_max)
-		s->f_kernel = false;
-	if (s->f_kernel && s->fplan.ok)
+	const int kind = kc_pick(s->kc);
+	if (kind == KK_F)
 		return launch_fscan(s, data, start, nbytes, final);
 	ScanArgs a;
 	a.data = data;
@@ -730,16 +603,16 @@ int launch_scan(dng_scan *s, const u8 *data, unsigned long long start,
 	a.tmpl = s->d_tmpl;
 	a.tmpl_bytes = s->tmpl_bytes;
 	a.wslice = DNG_W_SLICE_MAX;
-	cudaEvent_t e0 = get_event(s), e1 = get_event(s);
-	if (s->warp_kernel) {
-		const unsigned long long chunk = 32ull * s->wslice;
-		a.wslice = s->wslice;
+	cudaEvent_t e0 = get_event(s);
+	cudaEventRecord(e0, s->stream);
+	if (kind == KK_WARP) {
+		const unsigned long long chunk = 32ull * s->kc.wslice;
+		a.wslice = s->kc.wslice;
 		a.ntiles = (u32)((nbytes + chunk - 1) / chunk);
 		a.sslots = s->w_sslots;
 		a.s1slots = s->w_s1slots;
 		u32 grid = std::min<u32>((a.ntiles + DNG_NW - 1) / DNG_NW,
 		    (u32)s->sm_count);
-		cudaEventRecord(e0, s->stream);
 		scan_kernel_w<<<grid, DNG_NT, SMEM_W_FIXED + s->plan_bytes +
 		    s->tmpl_bytes + a.sslots * sizeof (SSlot) +
 		    a.s1slots * sizeof (SSlot1), s->stream>>>(a);
@@ -749,22 +622,11 @@ int launch_scan(dng_scan *s, const u8 *data, unsigned long long start,
 		a.s1slots = s->s1slots;
 		u32 grid = std::min<u32>(a.ntiles,
 		    (u32)s->sm_count * DNG_CTAS_PER_SM);
-		cudaEventRecord(e0, s->stream);
 		scan_kernel<<<grid, DNG_NT, SMEM_FIXED + s->plan_bytes +
 		    s->tmpl_bytes + a.sslots * sizeof (SSlot) +
 		    a.s1slots * sizeof (SSlot1), s->stream>>>(a);
 	}
-	cudaEventRecord(e1, s->stream);
-	if (!s->h_live && HOST_ALLOC(&s->h_live, NCTR * sizeof (unsigned long long))
-	    == cudaSuccess)
-		memset(s->h_live, 0, NCTR * sizeof (unsigned long long));
-	if (s->h_live)
-		cudaMemcpyAsync(s->h_live, s->d_counters,
-		    NCTR * sizeof (unsigned long long), cudaMemcpyDeviceToHost,
-		    s->stream);
-	s->ev_pairs.emplace_back(e0, e1);
-	s->launches++;
-	s->kernel_bytes += nbytes - start;
+	launched(s, e0, nbytes - start);
 	return s->cuda(cudaGetLastError(), "scan_kernel launch");
 }
 
@@ -938,98 +800,34 @@ int dng_scan_open(const dng_plan *plan, int device, dng_scan **out, char *err,
 			 * also covers the kernel's static shared variables */
 			per_cta = std::min(per_cta,
 			    (size_t)prop.sharedMemPerBlockOptin - 1024 - 512);
-			size_t used = SMEM_FIXED + s->plan_bytes + TMPL_RESERVE;
-			size_t room = per_cta > used ? per_cta - used : 0;
 			/* tier 1: 128 inline-key slots (64 when tight); tier 2:
-			 * as many compact slots as still fit (power of two) */
-			s->s1slots = room >= 24576 ? 256 : room >= 12288 ? 128 : 64;
-			size_t t1 = (size_t)s->s1slots * sizeof (SSlot1);
-			size_t left = room > t1 ? room - t1 : 0;
-			u32 n = DNG_SSLOTS_MIN;
-			while (n * 2 <= DNG_SSLOTS_MAX &&
-			    (size_t)n * 2 * sizeof (SSlot) <= left)
-				n *= 2;
-			s->sslots = n;
-			/* the per-warp kernel's fixed part differs: size its
-			 * tally cache separately */
+			 * as many compact slots as still fit.  The per-warp
+			 * kernel's fixed part differs: its own sizes */
+			size_t used = SMEM_FIXED + s->plan_bytes + TMPL_RESERVE;
 			size_t usedw = SMEM_W_FIXED + s->plan_bytes + TMPL_RESERVE;
+			size_t room = per_cta > used ? per_cta - used : 0;
 			size_t roomw = per_cta > usedw ? per_cta - usedw : 0;
+			s->s1slots = room >= 24576 ? 256 : room >= 12288 ? 128 : 64;
 			s->w_s1slots = roomw >= 24576 ? 256 : roomw >= 12288 ? 128 : 64;
-			size_t t1w = (size_t)s->w_s1slots * sizeof (SSlot1);
-			size_t leftw = roomw > t1w ? roomw - t1w : 0;
-			u32 nw = DNG_SSLOTS_MIN;
-			while (nw * 2 <= DNG_SSLOTS_MAX &&
-			    (size_t)nw * 2 * sizeof (SSlot) <= leftw)
-				nw *= 2;
-			s->w_sslots = nw;
-		}
-		/* a fan-out plan runs a long stage list per record and tallies
-		 * many tuples: it ran faster on CTA tiles (whose
-		 * warps move through the stages together and whose tally cache
-		 * is larger) than on per-warp chunks */
-		if (plan->dev.nmetrics > 1)
-			s->kernel_pref = 1;
-		if (const char *ev = getenv("DNG_KERNEL")) {
-			/* tuning/testing: force one kernel geometry */
-			s->kernel_pref = !strcmp(ev, "tile") ? 1 :
-			    !strcmp(ev, "warp") ? 2 : !strcmp(ev, "fast") ? 3 : 0;
-			s->warp_kernel = s->kernel_pref == 2;
+			s->sslots = tier2_slots(room - std::min(room,
+			    (size_t)s->s1slots * sizeof (SSlot1)));
+			s->w_sslots = tier2_slots(roomw - std::min(roomw,
+			    (size_t)s->w_s1slots * sizeof (SSlot1)));
 		}
 		/* the F path (fast.h), for the plans it models */
 		fplan_build(plan->dev, s->fplan);
-		/* start with 24 warps and the larger tally cache (f_nt): on an
-		 * H100 they scan faster than 28 warps on every BASELINE query, and
-		 * plans of three columns and more need the room for their keys */
-		s->f_nt = 768;
-		{
-			std::lock_guard<std::mutex> g(g_fnt_mu);
-			auto it = g_fnt_memo.find(fplan_hash(s->fplan));
-			if (it != g_fnt_memo.end()) {
-				s->f_nt = it->second;
-				s->f_probed = true;
-			}
-		}
-		if (const char *ev = getenv("DNG_F_WARPS")) {
-			s->f_nt = atoi(ev) >= 28 ? DNG_F_NT : 768;
-			s->f_probed = true;
-			s->f_forced = true;
-		}
-		if (getenv("DNG_FAST") && atoi(getenv("DNG_FAST")) == 0)
-			s->fplan.ok = 0;
 		if (const char *ev = getenv("DNG_JIT"))
 			s->jit_mode = !strcmp(ev, "sync") || !strcmp(ev, "wait") ? 2 :
 			    (!strcmp(ev, "0") || !strcmp(ev, "off")) ? 0 : 1;
-		if (s->kernel_pref == 3) {
-			/* forced: every eligible plan takes it, whatever the
-			 * templates cover; others choose as usual */
-			s->f_kernel = s->fplan.ok != 0;
-			if (!s->f_kernel)
-				s->kernel_pref = plan->dev.nmetrics > 1 ? 1 : 0;
-		}
 		s->f_smem_max = (u32)prop.sharedMemPerBlockOptin - 1024;
-		{
-			cudaError_t fe = cudaFuncSetAttribute(scan_kernel_f<7>,
+		cudaError_t fe = cudaFuncSetAttribute(scan_miss_kernel,
+		    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s->f_smem_max);
+		for (u32 nsl = 7, wb; nsl <= 13 && fe == cudaSuccess; nsl += 2)
+			fe = cudaFuncSetAttribute(fkernel(nsl, &wb),
 			    cudaFuncAttributeMaxDynamicSharedMemorySize,
 			    (int)s->f_smem_max);
-			if (fe == cudaSuccess)
-				fe = cudaFuncSetAttribute(scan_kernel_f<9>,
-				    cudaFuncAttributeMaxDynamicSharedMemorySize,
-				    (int)s->f_smem_max);
-			if (fe == cudaSuccess)
-				fe = cudaFuncSetAttribute(scan_kernel_f<11>,
-				    cudaFuncAttributeMaxDynamicSharedMemorySize,
-				    (int)s->f_smem_max);
-			if (fe == cudaSuccess)
-				fe = cudaFuncSetAttribute(scan_kernel_f<13>,
-				    cudaFuncAttributeMaxDynamicSharedMemorySize,
-				    (int)s->f_smem_max);
-			if (fe == cudaSuccess)
-				fe = cudaFuncSetAttribute(scan_miss_kernel,
-				    cudaFuncAttributeMaxDynamicSharedMemorySize,
-				    (int)s->f_smem_max);
-			if ((rc = s->cuda(fe, "cudaFuncSetAttribute")))
-				break;
-		}
+		if ((rc = s->cuda(fe, "cudaFuncSetAttribute")))
+			break;
 		if ((rc = s->cuda(cudaFuncSetAttribute(scan_kernel,
 		    cudaFuncAttributeMaxDynamicSharedMemorySize,
 		    (int)prop.sharedMemPerBlockOptin - 1024),
@@ -1051,14 +849,18 @@ int dng_scan_open(const dng_plan *plan, int device, dng_scan **out, char *err,
 			    std::to_string(prop.sharedMemPerBlockOptin) + ")");
 			break;
 		}
-		if (SMEM_W_FIXED + s->plan_bytes + TMPL_RESERVE +
-		    s->w_sslots * sizeof (SSlot) +
-		    s->w_s1slots * sizeof (SSlot1) >
-		    prop.sharedMemPerBlockOptin - 1024) {
-			/* no room for the per-warp geometry with this plan */
-			s->kernel_pref = 1;
-			s->warp_kernel = false;
-		}
+		/* (a plan with many capture rows leaves the F kernel's buffers
+		 * no room) */
+		u32 warp_bytes = 0;
+		fkernel(13, &warp_bytes);
+		const bool f_fits = fkernel_smem(warp_bytes, TMPL_RESERVE, 32,
+		    DNG_SSLOTS_MIN, s->fplan.nrows, DNG_F_NW) <= s->f_smem_max;
+		const bool warp_fits = SMEM_W_FIXED + s->plan_bytes + TMPL_RESERVE +
+		    s->w_sslots * sizeof (SSlot) + s->w_s1slots * sizeof (SSlot1) <=
+		    prop.sharedMemPerBlockOptin - 1024;
+		kc_open(s->kc, plan->dev.nmetrics > 1, s->fplan.ok != 0, f_fits,
+		    warp_fits, getenv("DNG_KERNEL"), getenv("DNG_FAST"),
+		    getenv("DNG_F_WARPS"));
 		if ((rc = s->cuda(cudaStreamCreateWithFlags(&s->stream,
 		    cudaStreamNonBlocking), "cudaStreamCreate")))
 			break;
@@ -1069,7 +871,7 @@ int dng_scan_open(const dng_plan *plan, int device, dng_scan **out, char *err,
 		if ((rc = s->cuda(DEV_ALLOC(s, &s->d_plan, sizeof (DevPlan) + 256),
 		    "cudaMalloc plan")))
 			break;
-		if (s->fplan.ok) {
+		if (s->kc.f_ok) {
 			if ((rc = s->cuda(DEV_ALLOC(s, &s->d_fplan, FPLAN_SMEM),
 			    "cudaMalloc fplan")))
 				break;
@@ -1424,22 +1226,6 @@ int dng_scan_feed_device(dng_scan *s, const void *devbuf, size_t len)
 		return 0;
 	}
 	cudaSetDevice(s->device);
-	/*
-	 * A large buffer would be ONE launch: nothing learnt from it could
-	 * help it.  Its head goes first, as a launch of its own, and what that
-	 * one counted (keys that overflowed the F kernel's tally cache: f_nt)
-	 * is looked at before the rest is launched.
-	 */
-	const size_t PROBE = (size_t)64 << 20;
-	if (!s->f_probed && s->fplan.ok && s->f_nt > 768 && len > 4 * PROBE) {
-		s->f_probed = true;
-		int rc = dng_scan_feed_device(s, devbuf, PROBE);
-		if (rc)
-			return rc;
-		CK(s, cudaStreamSynchronize(s->stream));
-		return dng_scan_feed_device(s, (const u8 *)devbuf + PROBE,
-		    len - PROBE);
-	}
 	const u8 *d = (const u8 *)devbuf;
 	s->bytes_fed += len;
 	/* locate the first and last newline (windows first, then all) */
@@ -1742,7 +1528,7 @@ int dng_scan_kernel_kind(const dng_scan *s)
 {
 	if (!s)
 		return DNG_EINVAL;
-	return s->f_kernel && s->fplan.ok ? 2 : s->warp_kernel ? 1 : 0;
+	return kc_pick(s->kc);
 }
 
 int dng_scan_jit_stats(dng_scan *s, int *state, uint64_t *launches,
@@ -1793,7 +1579,7 @@ int dng_scan_tally_stats(dng_scan *s, uint64_t *inline_overflow, int *f_warps)
 	if (inline_overflow)
 		*inline_overflow = c;
 	if (f_warps)
-		*f_warps = (int)(s->f_nt / 32);
+		*f_warps = (int)s->kc.f_nw;
 	return DNG_OK;
 }
 

@@ -32,6 +32,7 @@
 
 #include "plan.h"
 #include "tmpl.h"
+#include "kernel_choice.h"
 
 namespace dng {
 
@@ -40,9 +41,9 @@ enum : int {
 	F_POOL = 512, F_MAXKEY = 256,
 	F_MAXLINE = 4095,		/* longest line the F path matches */
 	F_MAXROWS = F_MAXPATHS + 2 * F_MAXCOLS,	/* capture rows: paths, ordinals */
-	F_NT = 896			/* most threads of the F kernels' CTA: 28
+	F_NT = 32 * DNG_F_NW		/* most threads of the F kernels' CTA: 28
 					 * warps of 72 registers; scans launch 24
-					 * unless DNG_F_WARPS=28 (api.cu) */
+					 * unless DNG_F_WARPS=28 (kernel_choice.h) */
 };
 
 /* offsets of the constant strings every FPlan pool starts with */

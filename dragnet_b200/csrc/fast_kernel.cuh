@@ -38,10 +38,8 @@
 namespace dng {
 
 #define DNG_F_NT F_NT			/* threads per CTA */
-#define DNG_F_NW (DNG_F_NT / 32)
 #define DNG_F_PRE 512			/* pre-lap bytes = longest straddling head */
 #define DNG_F_SLACK 64
-#define DNG_F_NLCAP 128			/* newline positions per chunk */
 #define DNG_F_MAXLINE DNG_F_PRE		/* host: sampled lines must be shorter */
 #define DNG_F_SEG 16			/* chunks per segment (at most) */
 
@@ -81,15 +79,15 @@ struct FWarpSmem {
 
 static constexpr u32 FPLAN_SMEM = (sizeof (FPlan) + 127) & ~127u;
 
-/* (nw = warps of the launch: DNG_F_NW, or fewer -- the capture rows keep
- * their stride -- when the tally cache needs the room) */
-template <int NSL>
-static inline size_t fkernel_smem(u32 tmpl_bytes, u32 s1slots, u32 sslots,
-    u32 nrows, u32 nw = DNG_F_NW)
+/* (warp_bytes = FWarpSmem<NSL>::BYTES; nw = warps of the launch: DNG_F_NW,
+ * or fewer -- the capture rows keep their stride -- when the tally cache
+ * needs the room) */
+static inline size_t fkernel_smem(u32 warp_bytes, u32 tmpl_bytes, u32 s1slots,
+    u32 sslots, u32 nrows, u32 nw)
 {
 	return FPLAN_SMEM + tmpl_bytes + (size_t)s1slots * sizeof (SSlot1) +
 	    (size_t)sslots * sizeof (SSlot) + (size_t)nrows * DNG_F_NT * 4 +
-	    (size_t)nw * FWarpSmem<NSL>::BYTES;
+	    (size_t)nw * warp_bytes;
 }
 
 /* mbarrier / TMA helpers on 32-bit shared addresses (no generic pointers to

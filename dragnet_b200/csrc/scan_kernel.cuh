@@ -36,6 +36,7 @@
 #include <cuda_runtime.h>
 #include "record.cuh"
 #include "tmpl.cuh"
+#include "kernel_choice.h"
 
 namespace dng {
 
@@ -1135,13 +1136,11 @@ scan_kernel(const ScanArgs a)
  */
 /* a chunk is 32 lane slices of a.wslice bytes (16 x an odd number, so that the
  * lanes' uint4 reads do not collide on banks); the host picks the slice that
- * puts just under 32 (or 64, ...) average records in a chunk */
-#define DNG_W_SLICE_MAX 208			/* 13 x 16 */
+ * puts just under 32 (or 64, ...) average records in a chunk (kernel_choice.h) */
 #define DNG_W_CHUNK (32 * DNG_W_SLICE_MAX)	/* largest chunk: 6656 bytes */
 #define DNG_W_PRELAP 768
 #define DNG_W_SLACK 64
 #define DNG_W_NLCAP 32				/* newline positions per pass */
-#define DNG_W_MAXLINE 512
 
 static constexpr size_t SMEM_W_BUF = DNG_W_PRELAP + DNG_W_CHUNK + DNG_W_SLACK;
 /* per warp: window, newline positions, fallback queue, mbarrier */

@@ -42,6 +42,7 @@ def build_hostcheck():
     deps = srcs + [os.path.join(CSRC, n) for n in
                    ('record.cuh', 'jsnum.cuh', 'jsdate.cuh', 'plan.h',
                     'result.h', 'tmpl.h', 'tmpl.cuh', 'fast.h', 'fast.cuh',
+                    'kernel_choice.h',
                     'fscan.cuh')]
     srcs.append(os.path.join(CSRC, 'jit.cpp'))
     deps += [os.path.join(CSRC, 'jit.cpp'), os.path.join(CSRC, 'jit.h'),

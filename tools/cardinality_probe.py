@@ -1,6 +1,6 @@
 """F kernel tally-cache adaptivity: a query with many keys (-b req.url,host) and
 one with few, with the CTA's warps forced (DNG_F_WARPS=28|24) or chosen by the
-library.  One device buffer per scan (so the probe launch decides)."""
+library.  One device buffer per scan."""
 import ctypes, os, sys, time
 R = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, R); sys.path.insert(0, os.path.join(R, 'tests'))
