@@ -6,14 +6,25 @@ Host-side mirror of the reference's Datasource interface for the scan path:
   lib/datasource-file.js:31-56  createDatasource / DatasourceFile fields
   lib/datasource-file.js:72-108 scan({query, dryRun})
   lib/datasource-file.js:124-192 scanInit (timeField check, dry run)
+  lib/datasource-file.js:307-433 build / indexScanImpl (fan-out scan)
+  lib/datasource-file.js:549-566 checkTimeArgs / checkIndexArgs
+  lib/datasource-file.js:573-618 query (index files -> points)
+  lib/datasource-file.js:729-746 indexRead
 The reference returns an object-mode stream of skinner points; here scan()
 returns a ScanResult holding the points, the per-stage counters and the list of
-files.  build/query/index* are outside the GPU hot path (SURVEY.md section 8)
-and raise NotImplementedError.
+files.  build() reads the raw data on the GPU and writes the sqlite indexes
+(index.py); query() and indexRead() never read raw data.
 """
 
+import json
+import time
+
+from . import index as mod_index
 from . import native
 from . import query as mod_query
+
+# Metrics one fan-out plan may hold (csrc/plan.h MAX_METRICS).
+MAX_METRICS = 8
 
 
 class DsError(Exception):
@@ -27,6 +38,8 @@ class ScanResult(object):
         self.files = files
         self.flat_counters = flat   # dng_counters as a dict
         self.stats = stats
+        self.index_files = None     # build(): the index files written
+        self.timing = None          # build(): {'scan_s', 'index_s'}
 
 
 def stage_counters(plan, c, npoints):
@@ -137,6 +150,7 @@ class DatasourceGpu(object):
         self.ds_timeformat = bc.get('timeFormat') or None
         self.ds_timefield = bc.get('timeField') or None
         self.ds_datapath = bc.get('path')
+        self.ds_indexpath = bc.get('indexPath') or None
         self.ds_filter = dsconfig.get('filter') or None
         self.ds_device = dsconfig.get('device', 0)
         # (root, timeFormat, after_ms, before_ms) -> [paths]: the reference's
@@ -169,12 +183,52 @@ class DatasourceGpu(object):
                                    data_format=self.ds_format)
         return run_plan(plan, files=files, device=self.ds_device)
 
+    def checkTimeArgs(self, args):
+        """lib/datasource-file.js:549-556."""
+        after, before = args.get('timeAfter'), args.get('timeBefore')
+        if after is not None and before is None:
+            return DsError('cannot specify --after without --before')
+        if before is not None and after is None:
+            return DsError('cannot specify --before without --after')
+        return None
+
+    def checkIndexArgs(self, args, needsindex, needstime):
+        """lib/datasource-file.js:558-566."""
+        if needsindex and self.ds_indexpath is None:
+            return DsError('datasource is missing "indexpath"')
+        if needstime and args['interval'] != 'all' and \
+                self.ds_timefield is None:
+            return DsError('datasource is missing "timefield"')
+        return None
+
+    def _fanout(self, metrics, interval, after, before, files):
+        """Every metric over the raw data, each point tagged ('__dn_metric',
+        i).  A plan holds at most MAX_METRICS metrics, so more are computed in
+        passes of that many, and each pass reads the input again."""
+        queries = [mod_query.metricQuery(m, after, before, interval,
+                                         self.ds_timefield)
+                   for m in metrics]
+        pts, counters, flats, stats = [], [], [], []
+        for base in range(0, len(queries), MAX_METRICS):
+            plan = mod_query.scan_plan_multi(
+                queries[base:base + MAX_METRICS], ds_filter=self.ds_filter,
+                time_field=self.ds_timefield, data_format=self.ds_format)
+            r = run_plan(plan, files=files, device=self.ds_device)
+            for fields, value in r.points:
+                fields[-1] = ('__dn_metric', base + fields[-1][1])
+                pts.append((fields, value))
+            counters += r.counters
+            flats += r.flat_counters
+            stats.append(r.stats)
+        return ScanResult(pts, counters, list(files), flats,
+                          stats[0] if len(stats) == 1 else stats)
+
     def indexScan(self, args):
         """The scan half of build/index-scan (lib/datasource-file.js:321-433):
-        one pass over the raw data computing every metric; returns the points
-        an IndexSink would store, each tagged ('__dn_metric', i).  args:
-        metrics [{'filter', 'breakdowns'}], interval, dryRun, timeAfter,
-        timeBefore (ms)."""
+        one pass over the raw data computing every metric (one pass per
+        MAX_METRICS metrics); returns the points an IndexSink would store,
+        each tagged ('__dn_metric', i).  args: metrics [{'filter',
+        'breakdowns'}], interval, dryRun, timeAfter, timeBefore (ms)."""
         after, before = args.get('timeAfter'), args.get('timeBefore')
         if self.ds_timefield is None and (args['interval'] != 'all' or
                                           after or before):
@@ -185,20 +239,113 @@ class DatasourceGpu(object):
                              after, before)
         if args.get('dryRun'):
             return ScanResult([], {}, files)
-        queries = [mod_query.metricQuery(m, after, before, args['interval'],
-                                         self.ds_timefield)
-                   for m in args['metrics']]
-        plan = mod_query.scan_plan_multi(queries, ds_filter=self.ds_filter,
-                                         time_field=self.ds_timefield,
-                                         data_format=self.ds_format)
-        return run_plan(plan, files=files, device=self.ds_device)
+        return self._fanout(args['metrics'], args['interval'], after, before,
+                            files)
 
-    def build(self, *a, **k):
-        raise NotImplementedError('writing sqlite indexes stays on the '
-                                  'reference path (IndexSink); use indexScan '
-                                  'for the points')
+    def build(self, args):
+        """`dn build` (lib/datasource-file.js:307-433): the fan-out scan of
+        every metric on the GPU, with the datasource filter applied, then
+        the points into the index files of args['interval'] under the
+        datasource's indexPath.  args: metrics (configuration form, each with
+        a 'name'), interval ('all', 'hour' or 'day'), dryRun, timeAfter,
+        timeBefore (ms).  A dry run only lists the input files.  Returns a
+        ScanResult whose .index_files are the files written and whose
+        .timing splits the wall time into the scan and the sqlite writes."""
+        after, before = args.get('timeAfter'), args.get('timeBefore')
+        err = self.checkTimeArgs(args) or \
+            self.checkIndexArgs(args, True, True)
+        if err is not None:
+            return err
+        if args['interval'] not in ('all',) + tuple(mod_index.INTERVALS):
+            return DsError('unsupported interval: "%s"' % args['interval'])
+        if self.ds_format not in ('json', 'json-skinner'):
+            return DsError('unsupported format: "%s"' % self.ds_format)
+        if self.ds_find is None:
+            return DsError('no file enumerator ("findFiles")')
+        files = self.ds_find(self.ds_datapath, self.ds_timeformat,
+                             after, before)
+        if args.get('dryRun'):
+            return ScanResult([], {}, files)
+        t0 = time.perf_counter()
+        res = self._fanout(args['metrics'], args['interval'], after, before,
+                           files)
+        t1 = time.perf_counter()
+        written = mod_index.write_index(self.ds_indexpath, args['metrics'],
+                                        args['interval'], res.points)
+        if isinstance(written, Exception):
+            return DsError(str(written))
+        res.index_files = written
+        res.timing = {'scan_s': t1 - t0,
+                      'index_s': time.perf_counter() - t1}
+        return res
 
-    query = indexRead = build
+    def query(self, args):
+        """`dn query` (lib/datasource-file.js:573-618): the index files of
+        args['interval'] (default 'all') that the query's time bounds
+        select, the query run against each, and the rows of all of them
+        aggregated as the query asks.  The counters are the reference's
+        'Index List' and 'Index Result Aggregator' stage counters."""
+        query = args['query']
+        err = self.checkTimeArgs(args) or \
+            self.checkIndexArgs(args, True, False)
+        if err is not None:
+            return err
+        fp = mod_index.indexFindParams(args.get('interval') or 'all',
+                                       self.ds_indexpath, query.qc_after,
+                                       query.qc_before)
+        if isinstance(fp, Exception):
+            return DsError(str(fp))
+        if self.ds_find is None:
+            return DsError('no file enumerator ("findFiles")')
+        files = self.ds_find(fp['root'], fp['timeformat'], fp['after'],
+                             fp['before'])
+        if args['dryRun']:
+            return ScanResult([], {}, files)
+        r = mod_index.query_indexes(files, query)
+        if isinstance(r, Exception):
+            return DsError(str(r))
+        points, counters = r
+        return ScanResult(points, counters, files)
+
+    def indexRead(self, args):
+        """`dn index-read` (lib/datasource-file.js:729-746): json-skinner
+        points that already carry fields.__dn_metric (args['input']: bytes,
+        or an iterable of lines) into the index files of args['interval'],
+        stored as they are, without aggregating them again.  Lines that are
+        not JSON are skipped, as the reference's json-skinner parser drops
+        them.  Returns the files written."""
+        if args['interval'] not in ('all',) + tuple(mod_index.INTERVALS):
+            return DsError('unsupported interval: "%s"' % args['interval'])
+        err = self.checkIndexArgs(args, True, False)
+        if err is not None:
+            return err
+        data = args['input']
+        lines = data.split(b'\n') if isinstance(data, bytes) else data
+        points = []
+        nmetrics = len(args['metrics'])
+        for line in lines:
+            if isinstance(line, bytes):
+                line = line.decode('utf-8', 'replace')
+            if not line.strip():
+                continue
+            try:
+                p = json.loads(line)
+            except ValueError:
+                continue
+            if not isinstance(p, dict) or \
+                    not isinstance(p.get('fields'), dict):
+                continue
+            mi = p['fields'].get('__dn_metric')
+            if not isinstance(mi, int) or isinstance(mi, bool) or \
+                    not 0 <= mi < nmetrics:
+                return DsError('point without a valid "__dn_metric": %s'
+                               % line.strip())
+            points.append((p['fields'], p.get('value')))
+        written = mod_index.write_index(self.ds_indexpath, args['metrics'],
+                                        args['interval'], points)
+        if isinstance(written, Exception):
+            return DsError(str(written))
+        return written
 
 
 def createDatasource(args):

@@ -4,12 +4,19 @@
  * the scan() of the reference's file datasource (lib/datasource-file.js:72-108;
  * backend dispatch lib/dragnet.js:296-303).
  *
- *   scanOpen(planJson, device)  -> scan object (throws Error on DNG_E*)
+ *   scanOpen(planJson, device, breakdownNames[, tagMetric])
+ *                               -> scan object (throws Error on DNG_E*)
+ *                                  For a fan-out plan ("metrics": [...], the
+ *                                  scan of `dn build`), breakdownNames holds
+ *                                  every metric's names one metric after the
+ *                                  other, and a true tagMetric adds
+ *                                  fields.__dn_metric to each point.
  *   scan.feed(buffer, cb)          dng_scan_feed      (bytes are consumed)
  *   scan.feedFile(path, cb)        dng_scan_feed_file
  *   scan.finish(cb)             -> cb(err, points, counters)
  *                                  points   = [{fields: {name: string|number},
  *                                              value: N}, ...]
+ *                                  (counters: of the plan's first metric)
  *                                  counters = {lines, invalid_json, ...}
  *   scan.close()                   dng_scan_destroy + dng_plan_destroy
  *
@@ -37,6 +44,7 @@ struct ScanWrap {
 	dng_plan *plan = nullptr;
 	dng_scan *scan = nullptr;
 	std::vector<std::string> names;		/* breakdown names, in order */
+	bool tag = false;		/* fan-out: set fields.__dn_metric */
 };
 
 void Throw(napi_env env, const char *msg)
@@ -104,6 +112,13 @@ napi_value Points(napi_env env, Work *k)
 {
 	const size_t n = dng_result_count(k->res);
 	const size_t nc = dng_result_ncols(k->res);
+	/* metric m's names start at first[m] in the names given to scanOpen */
+	const size_t nm = dng_result_nmetrics(k->res);
+	std::vector<size_t> first(nm + 1, 0), ncm(nm, 0);
+	for (size_t m = 0; m < nm; m++) {
+		ncm[m] = dng_result_ncols_metric(k->res, (int)m);
+		first[m + 1] = first[m] + ncm[m];
+	}
 	napi_value arr;
 	napi_create_array_with_length(env, n, &arr);
 	std::vector<const char *> strs(nc);
@@ -114,10 +129,14 @@ napi_value Points(napi_env env, Work *k)
 		uint64_t value = 0;
 		dng_result_get(k->res, i, strs.data(), lens.data(), isnum.data(),
 		    nums.data(), &value);
+		const int m = dng_result_metric(k->res, i);
+		const size_t base = m >= 0 && (size_t)m < nm ? first[m] : 0;
+		const size_t ncols = m >= 0 && (size_t)m < nm ? ncm[m] : nc;
 		napi_value pt, fields, v;
 		napi_create_object(env, &pt);
 		napi_create_object(env, &fields);
-		for (size_t j = 0; j < nc && j < k->w->names.size(); j++) {
+		for (size_t j = 0; j < ncols && base + j < k->w->names.size();
+		    j++) {
 			/* discrete values are strings, bucketized ones the
 			 * bucket minimum as a number (tst.scan_file.sh.out:86) */
 			if (isnum[j])
@@ -125,7 +144,12 @@ napi_value Points(napi_env env, Work *k)
 			else
 				napi_create_string_utf8(env, strs[j], lens[j], &v);
 			napi_set_named_property(env, fields,
-			    k->w->names[j].c_str(), v);
+			    k->w->names[base + j].c_str(), v);
+		}
+		if (k->w->tag) {
+			/* lib/datasource-file.js:412-419 */
+			napi_create_double(env, (double)m, &v);
+			napi_set_named_property(env, fields, "__dn_metric", v);
 		}
 		napi_set_named_property(env, pt, "fields", fields);
 		napi_create_double(env, (double)value, &v);
@@ -278,11 +302,11 @@ void Finalize(napi_env, void *data, void *)
 	delete w;
 }
 
-/* scanOpen(planJson, device, breakdownNames) */
+/* scanOpen(planJson, device, breakdownNames[, tagMetric]) */
 napi_value ScanOpen(napi_env env, napi_callback_info info)
 {
-	size_t argc = 3;
-	napi_value argv[3], obj, fn;
+	size_t argc = 4;
+	napi_value argv[4], obj, fn;
 	if (napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr) !=
 	    napi_ok || argc < 3) {
 		Throw(env, "scanOpen(planJson, device, breakdownNames)");
@@ -299,6 +323,10 @@ napi_value ScanOpen(napi_env env, napi_callback_info info)
 		napi_get_element(env, argv[2], i, &e);
 		w->names.push_back(GetString(env, e));
 	}
+	int32_t tag = 0;
+	if (argc >= 4)
+		napi_get_value_int32(env, argv[3], &tag);
+	w->tag = tag != 0;
 	char err[512];
 	err[0] = '\0';
 	int rc = dng_plan_create(plan.c_str(), &w->plan, err, sizeof (err));

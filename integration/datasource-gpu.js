@@ -4,8 +4,10 @@
  *
  * NOT EXECUTED IN THIS REPOSITORY: node is not installed in the build image.
  * It is the reference-side half of the drop-in boundary and mirrors
- * lib/datasource-file.js:31-108 of the reference; everything except scan()
- * delegates to the file backend.  Add to lib/dragnet.js:datasourceForConfig:
+ * lib/datasource-file.js:31-108 and :307-433 of the reference: scan(), and
+ * the raw-data pass of build() and indexScan(), run on the GPU; query() and
+ * indexRead(), which read only index files and points, stay on the file
+ * backend.  Add to lib/dragnet.js:datasourceForConfig:
  *
  *     if (bename == 'gpu')
  *             return (mod_datasource_gpu.createDatasource(args));
@@ -13,6 +15,7 @@
 
 var mod_assertplus = require('assert-plus');
 var mod_stream = require('stream');
+var mod_vasync = require('vasync');
 var mod_vstream = require('vstream');
 var VError = require('verror');
 
@@ -28,7 +31,7 @@ exports.createDatasource = function createDatasource(args)
 	if (typeof (args.dsconfig.ds_backend_config.path) != 'string')
 		return (new VError('expected datasource "path" to be a string'));
 
-	/* build/query/index* stay on the file backend */
+	/* query/indexRead and the index files stay on the file backend */
 	filecfg = Object.create(args.dsconfig);
 	filecfg.ds_backend = 'file';
 	fileds = mod_datasource_file.createDatasource(
@@ -48,7 +51,10 @@ function DatasourceGpu(args, fileds)
 	this.ds_log = args.log;
 }
 
-[ 'close', 'build', 'query', 'indexScan', 'indexRead' ].forEach(function (m) {
+/* metrics one fan-out plan may hold (MAX_METRICS, csrc/plan.h) */
+var MAX_METRICS = 8;
+
+[ 'close', 'query', 'indexRead' ].forEach(function (m) {
 	DatasourceGpu.prototype[m] = function () {
 		return (this.ds_file[m].apply(this.ds_file, arguments));
 	};
@@ -62,7 +68,7 @@ DatasourceGpu.prototype.scan = function (args)
 {
 	var self = this;
 	var query = args.query;
-	var scanctx, plan, scan, out, synthetic, bounds, tf;
+	var scanctx, plan, scan, out;
 
 	/* file enumeration, --dry-run and the timeField check are unchanged */
 	scanctx = this.ds_file.scanInit({
@@ -75,25 +81,10 @@ DatasourceGpu.prototype.scan = function (args)
 		return (scanctx.outstream);
 
 	/* the plan JSON is just the QueryConfig + datasource properties */
-	synthetic = query.qc_synthetic.map(function (s) {
-		return ({ 'name': s.name, 'field': s.field });
-	});
-	bounds = null;
-	/* (as lib/stream-scan.js:62: either bound asks for the time filter) */
-	if (query.qc_before !== null || query.qc_after !== null) {
-		synthetic.push({ 'name': 'dn_ts', 'field': this.ds_timefield });
-		tf = mod_dragnet_impl.queryTimeBoundsFilter(query, 'dn_ts');
-		bounds = { 'field': 'dn_ts',
-		    'ge': tf.and[0].ge[1], 'lt': tf.and[1].lt[1] };
-	}
-	plan = JSON.stringify({
-	    'format': this.ds_format,
-	    'ds_filter': this.ds_filter,
-	    'filter': query.qc_filter,
-	    'synthetic': synthetic,
-	    'time_bounds': bounds,
-	    'breakdowns': query.qc_breakdowns
-	});
+	plan = queryPlan(query, this.ds_timefield);
+	plan.format = this.ds_format;
+	plan.ds_filter = this.ds_filter;
+	plan = JSON.stringify(plan);
 
 	out = mod_vstream.wrapStream(new mod_stream.PassThrough(
 	    { 'objectMode': true, 'highWaterMark': 0 }), 'Aggregator');
@@ -131,4 +122,213 @@ DatasourceGpu.prototype.scan = function (args)
 		});
 	});
 	return (out);
+};
+
+/*
+ * What a scan of one query computes: its filter, synthetic date fields, time
+ * bounds and breakdowns, as the plan JSON names them.
+ */
+function queryPlan(query, timefield)
+{
+	var synthetic, bounds, tf;
+
+	synthetic = query.qc_synthetic.map(function (s) {
+		return ({ 'name': s.name, 'field': s.field });
+	});
+	bounds = null;
+	/* (as lib/stream-scan.js:62: either bound asks for the time filter) */
+	if (query.qc_before !== null || query.qc_after !== null) {
+		synthetic.push({ 'name': 'dn_ts', 'field': timefield });
+		tf = mod_dragnet_impl.queryTimeBoundsFilter(query, 'dn_ts');
+		bounds = { 'field': 'dn_ts',
+		    'ge': tf.and[0].ge[1], 'lt': tf.and[1].lt[1] };
+	}
+	return ({
+	    'filter': query.qc_filter,
+	    'synthetic': synthetic,
+	    'time_bounds': bounds,
+	    'breakdowns': query.qc_breakdowns
+	});
+}
+
+/*
+ * build(): same contract as DatasourceFile.build (lib/datasource-file.js:
+ * 307-320): the datasource filter applies, the points go into the file
+ * backend's own index sink.
+ */
+DatasourceGpu.prototype.build = function (args, callback)
+{
+	var scanargs, key;
+
+	mod_assertplus.ok(!args.hasOwnProperty('sink'));
+	mod_assertplus.ok(!args.hasOwnProperty('filter'));
+	scanargs = {};
+	for (key in args)
+		scanargs[key] = args[key];
+	scanargs.filter = this.ds_filter;
+	return (this.indexScanImpl(scanargs, callback));
+};
+
+/*
+ * indexScan(): same contract as DatasourceFile.indexScan (:698-723): the
+ * tagged points, into a PassThrough instead of index files.
+ */
+DatasourceGpu.prototype.indexScan = function (args)
+{
+	var sink = new mod_stream.PassThrough({
+	    'objectMode': true,
+	    'highWaterMark': 128
+	});
+
+	this.indexScanImpl({
+	    'dryRun': false,
+	    'filter': args.filter,
+	    'interval': args.interval,
+	    'metrics': args.metrics,
+	    'sink': sink,
+	    'timeAfter': args.timeAfter,
+	    'timeBefore': args.timeBefore
+	}, function (err) {
+		if (err)
+			sink.emit('error', err);
+	});
+	return (sink);
+};
+
+/*
+ * The raw-data pass of build and indexScan (lib/datasource-file.js:322-433):
+ * one fan-out scan computes every metric, and each point is written to the
+ * sink tagged fields.__dn_metric.  A plan holds at most MAX_METRICS metrics,
+ * so more are computed in passes of that many; each pass reads the input
+ * files again.
+ */
+DatasourceGpu.prototype.indexScanImpl = function (args, callback)
+{
+	var self = this;
+	var fileds = this.ds_file;
+	var error, scanctx, sink, queries, passes, paths, i;
+
+	mod_assertplus.arrayOfObject(args.metrics, 'args.metrics');
+	mod_assertplus.bool(args.dryRun, 'args.dryRun');
+	mod_assertplus.string(args.interval, 'args.interval');
+
+	error = fileds.checkTimeArgs(args);
+	if (error === null)
+		error = fileds.checkIndexArgs(args, args.sink === undefined, true);
+	if (error === null) {
+		/* (the datasource filter goes into the plan) */
+		scanctx = fileds.scanInit({
+		    'filter': null,
+		    'dryRun': args.dryRun,
+		    'timeAfter': args.timeAfter,
+		    'timeBefore': args.timeBefore
+		});
+		if (scanctx instanceof Error)
+			error = scanctx;
+	}
+	if (error !== null) {
+		setImmediate(callback, error);
+		return (null);
+	}
+	if (args.dryRun) {
+		scanctx.outstream.on('end', callback);
+		scanctx.outstream.on('data', function () {});
+		return (scanctx.outstream);
+	}
+
+	sink = args.sink || fileds.indexSink({
+	    'metrics': args.metrics,
+	    'interval': args.interval
+	});
+	if (sink instanceof Error) {
+		setImmediate(callback, sink);
+		return (null);
+	}
+
+	queries = args.metrics.map(function (m) {
+		return (mod_dragnet_impl.metricQuery(m, args.timeAfter,
+		    args.timeBefore, args.interval, self.ds_timefield));
+	});
+	passes = [];
+	for (i = 0; i < queries.length; i += MAX_METRICS)
+		passes.push(i);
+
+	paths = [];
+	scanctx.findstream.on('data', function (fileinfo) {
+		if (!fileinfo.error)
+			paths.push(fileinfo.path);
+	});
+	scanctx.findstream.on('end', function () {
+		mod_vasync.forEachPipeline({
+		    'inputs': passes,
+		    'func': function (base, passcb) {
+			self.fanoutPass(queries.slice(base, base + MAX_METRICS),
+			    base, args.filter || null, paths, sink, passcb);
+		    }
+		}, function (err) {
+			if (err) {
+				callback(err);
+				return;
+			}
+			if (args.sink) {
+				sink.end();
+				callback();
+				return;
+			}
+			sink.on('flushed', callback);
+			sink.end();
+		});
+	});
+	return (sink);
+};
+
+/*
+ * One fan-out scan of up to MAX_METRICS queries over the files; its points
+ * are written to the sink with __dn_metric renumbered from "base".
+ */
+DatasourceGpu.prototype.fanoutPass = function (queries, base, dsfilter, paths,
+    sink, callback)
+{
+	var names, plan, scan;
+
+	names = [];
+	queries.forEach(function (q) {
+		q.qc_breakdowns.forEach(function (b) { names.push(b.name); });
+	});
+	plan = JSON.stringify({
+	    'format': this.ds_format,
+	    'ds_filter': dsfilter,
+	    'metrics': queries.map(
+		function (q) { return (queryPlan(q, this.ds_timefield)); },
+		this)
+	});
+
+	try {
+		scan = dragnet_gpu.scanOpen(plan, this.ds_device, names, 1);
+	} catch (ex) {
+		setImmediate(callback, ex);
+		return;
+	}
+	mod_vasync.forEachPipeline({
+	    'inputs': paths,
+	    'func': function (path, feedcb) { scan.feedFile(path, feedcb); }
+	}, function (err) {
+		if (err) {
+			scan.close();
+			callback(err);
+			return;
+		}
+		scan.finish(function (ferr, points) {
+			scan.close();
+			if (ferr) {
+				callback(ferr);
+				return;
+			}
+			points.forEach(function (p) {
+				p.fields.__dn_metric += base;
+				sink.write(p);
+			});
+			callback();
+		});
+	});
 };
