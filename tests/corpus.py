@@ -3,8 +3,11 @@ parity tests.  Everything here is checked oracle-vs-implementation, so the
 cases may go beyond what the reference's own tests exercise (those are in
 tests/golden)."""
 
+import decimal
 import json
+import math
 import random
+import struct
 
 from hostmirror import dn as mod_dn
 from dragnet_b200 import query as mod_query
@@ -142,49 +145,86 @@ def random_lines(seed, n):
 # query plans
 # ---------------------------------------------------------------------------
 
-def make_plan(argv, ds=None):
-    """`dn scan ARGV` against datasource properties ds -> plan dict."""
+class DroppedBreakdown(ValueError):
+    pass
+
+
+def written_breakdowns(argv):
+    """The field names written after each -b of argv: the text split at
+    commas outside [...], each piece without its [...] attributes."""
+    names = []
+    for i in range(1, len(argv)):
+        if argv[i - 1] not in ('-b', '--breakdowns'):
+            continue
+        depth, piece = 0, ''
+        for ch in argv[i] + ',':
+            if ch == '[':
+                depth += 1
+            elif ch == ']':
+                depth -= 1
+            elif ch == ',' and depth == 0:
+                if piece:
+                    names.append(piece)
+                piece = ''
+            elif depth == 0:
+                piece += ch
+    return names
+
+
+def make_plan(argv, ds=None, allow_dropped=False):
+    """`dn scan ARGV` against datasource properties ds -> plan dict.
+
+    dn's breakdown parser drops a trailing bare name of one character (`-b a`
+    groups by nothing, `-b a,b` by a alone; lib/attr-parser.js:73 tests
+    `j < str.length - 1`).  A query that means to group by such a name must
+    end it with a comma (`-b a,`); one that loses a name raises
+    DroppedBreakdown unless allow_dropped is set."""
     ds = ds or {}
     options = mod_dn.dnParseArgs(list(argv))
     q = mod_dn.dnQueryConfig(options)['query']
-    return mod_query.scan_plan(q, ds_filter=ds.get('filter'),
+    plan = mod_query.scan_plan(q, ds_filter=ds.get('filter'),
                                time_field=ds.get('timeField'),
                                data_format=ds.get('dataFormat', 'json'))
+    got = [b['name'] for b in plan['breakdowns']]
+    want = written_breakdowns(argv)
+    if got != want and not allow_dropped:
+        raise DroppedBreakdown('%r groups by %r, not by %r' % (argv, got, want))
+    return plan
 
 
 EDGE_QUERIES = [
     ([], None),
-    (['-b', 'a'], None),
+    (['-b', 'a,'], None),
     (['-b', 'a.b'], None),
     (['-b', 'a.b.c'], None),
-    (['-b', 'a,b'], None),
+    (['-b', 'a,b,'], None),
     (['-b', 'a[aggr=quantize]'], None),
     (['-b', 'a[aggr=lquantize,step=100]'], None),
-    (['-b', 'b[aggr=lquantize,step=7],a'], None),
+    (['-b', 'b[aggr=lquantize,step=7],a,'], None),
     (['-b', 'a.b[aggr=quantize],req.method'], None),
     (['-f', '{"eq":["a",200]}'], None),
-    (['-f', '{"eq":["a","200"]}', '-b', 'a'], None),
-    (['-f', '{"ne":["a",5]}', '-b', 'a'], None),
-    (['-f', '{"lt":["a",100]}', '-b', 'a'], None),
-    (['-f', '{"ge":["a","abc"]}', '-b', 'a'], None),
-    (['-f', '{"le":["a","5"]}', '-b', 'a'], None),
+    (['-f', '{"eq":["a","200"]}', '-b', 'a,'], None),
+    (['-f', '{"ne":["a",5]}', '-b', 'a,'], None),
+    (['-f', '{"lt":["a",100]}', '-b', 'a,'], None),
+    (['-f', '{"ge":["a","abc"]}', '-b', 'a,'], None),
+    (['-f', '{"le":["a","5"]}', '-b', 'a,'], None),
     (['-f', '{"gt":["a.b",1]}', '-b', 'a.b'], None),
-    (['-f', '{"eq":["a",true]}', '-b', 'a'], None),
+    (['-f', '{"eq":["a",true]}', '-b', 'a,'], None),
     (['-f', '{"eq":["a.b","1,2"]}', '-b', 'a.b'], None),
     (['-f', '{"eq":["a","[object Object]"]}'], None),
-    (['-f', '{"and":[{"ge":["a",1]},{"lt":["a",300]}]}', '-b', 'a'], None),
-    (['-f', '{"or":[{"eq":["a","x"]},{"eq":["b",2]}]}', '-b', 'a,b'], None),
+    (['-f', '{"and":[{"ge":["a",1]},{"lt":["a",300]}]}', '-b', 'a,'], None),
+    (['-f', '{"or":[{"eq":["a","x"]},{"eq":["b",2]}]}', '-b', 'a,b,'], None),
     (['-f', '{"or":[{"and":[{"eq":["a",1]},{"eq":["b",1]}]},{"gt":["a",100]}]}'],
      None),
     (['-f', '{"eq":["req.method","GET"]}', '-b', 'req.method'],
      {'filter': {'ne': ['a', 1]}}),
     (['-b', 'ts[date,field=t,aggr=lquantize,step=86400]'], None),
-    (['-b', 'ts[date,field=t],a'], None),
-    (['-b', 'a', '--after', '2014-04-30', '--before', '2014-05-02'],
+    (['-b', 'ts[date,field=t],a,'], None),
+    (['-b', 'a,', '--after', '2014-04-30', '--before', '2014-05-02'],
      {'timeField': 't'}),
-    (['-b', 't[date],a'], None),
+    (['-b', 't[date],a,'], None),
     (['-b', 'a[date,field=t]'], None),
-    (['-b', '[aggr=quantize]x'], None) if False else (['-b', 'x'], None),
+    (['-b', 'x,'], None),
     (['-b', ''], None) if False else (['-b', 'length'], None),
     (['-b', 'a.0'], None),
     (['-b', 'a.b.1,a.b.length'], None),
@@ -196,10 +236,10 @@ EDGE_QUERIES = [
 
 SKINNER_QUERIES = [
     ([], {'dataFormat': 'json-skinner'}),
-    (['-b', 'a'], {'dataFormat': 'json-skinner'}),
+    (['-b', 'a,'], {'dataFormat': 'json-skinner'}),
     (['-b', 'req.method'], {'dataFormat': 'json-skinner'}),
-    (['-b', 'a.b,b'], {'dataFormat': 'json-skinner'}),
-    (['-f', '{"eq":["a",1]}', '-b', 'a'], {'dataFormat': 'json-skinner'}),
+    (['-b', 'a.b,b,'], {'dataFormat': 'json-skinner'}),
+    (['-f', '{"eq":["a",1]}', '-b', 'a,'], {'dataFormat': 'json-skinner'}),
 ]
 
 BASELINE_QUERIES = {
@@ -631,3 +671,377 @@ def weight_sums(lines):
         k = doc['fields']['key'].encode()
         sums[k] = sums.get(k, 0) + int(v)
     return sums
+
+
+# ---------------------------------------------------------------------------
+# value sweep (tests/test_value_sweep_host.py, test_gpu_value_sweep.py): a few
+# record shapes, each field a value where JS semantics are easy to get wrong.
+# Lines are 120-200 bytes, so that the F kernel keeps its chunks (at most 128
+# lines) and learns the shapes as templates.
+# ---------------------------------------------------------------------------
+
+TWO53 = 1 << 53
+# steps of the lquantize queries: every m * step and its neighbouring doubles
+# are numbers of the sweep
+SWEEP_STEPS = [1, 7, 100, 2147483647, -3, 3600, 86400]
+# a number of the sweep the relational filters compare with (with its two
+# neighbours, also numbers of the sweep)
+SWEEP_CONST = 1234.5678
+# code points at the UTF-8 (1/2/3/4 bytes) and UTF-16 (surrogates) edges
+SWEEP_CPS = [0x41, 0x7a, 0x7f, 0x80, 0xe9, 0x7ff, 0x800, 0xd7ff, 0xe000,
+             0xff61, 0xfffd, 0xffff, 0x10000, 0x1f600, 0x10ffff]
+SWEEP_NSTR = ['26', ' 26 ', '\u00a026\ufeff', '\ufeff26', '\u300026', '-0',
+              '0', '', ' ', '1e3', '1E+3', '.5', '5.', '+5', '-5', '0x1F',
+              '0X1f', '0o17', '0b101', '0x', '0b2', 'Infinity', '-Infinity',
+              '+Infinity', 'infinity', 'NaN', 'abc', '12abc', '1_000', '--5',
+              '9007199254740993', '1e309', '-1e309', '5e-324',
+              '00026', '2.6e1', '26.000', '0.1', '\u00a0', '\u2028-7\u2029']
+
+
+def _f64(u):
+    return struct.unpack('<d', struct.pack('<Q', u))[0]
+
+
+def sweep_number(rng):
+    """The text of a bare JSON number."""
+    c = rng.randrange(10)
+    if c == 0:
+        nd = rng.randint(1, 20)
+        v = rng.randrange(10 ** (nd - 1) if nd > 1 else 0, 10 ** nd)
+        return ('-' if rng.random() < 0.3 else '') + str(v)
+    if c == 1:
+        # 16-digit integers above 2^53: their key is JS String(value), not
+        # their own digits
+        return str(rng.randrange(TWO53 + 1, 10 ** 16))
+    if c == 2:
+        return rng.choice([str(TWO53 - 1), str(TWO53), str(TWO53 + 1),
+                           str(TWO53 + 2), str(TWO53 + 3), '-' + str(TWO53 + 1),
+                           '-' + str(TWO53 - 1), '-0', '0', '0.0', '-0.0',
+                           '0e0', '-0e-0', '1.7976931348623157e308',
+                           '1.7976931348623158e308', '1e309', '-1e309',
+                           '5e-324', '2.5e-324', '2.4703282292062328e-324',
+                           '2.2250738585072014e-308', '2.225073858507201e-308',
+                           '123456789012345', '-123456789012345',
+                           '999999999999999', '1000000000000000',
+                           '1e21', '1e-7', '100000000000000000000'])
+    if c == 3:
+        # a random binary64: shortest repr, or 17-25 significant digits
+        while True:
+            x = _f64(rng.getrandbits(64))
+            if math.isfinite(x):
+                break
+        if rng.random() < 0.5:
+            return repr(x)
+        return '%.*e' % (rng.randint(16, 24), x)
+    if c == 4:
+        # exponent spellings: E+, e-, trailing zeros, leading fraction zeros
+        m = rng.randrange(1, 10 ** rng.randint(1, 6))
+        e = rng.randint(-30, 30)
+        return rng.choice(['%dE+%d', '%de-%d', '%d.000e%d', '%d00E-%d',
+                           '0.000%de%d']) % (m, abs(e))
+    if c == 5:
+        # halfway between two neighbouring doubles, written out exactly
+        k = rng.randint(40, 75)
+        a = _f64(rng.randrange(1 << 52) | (1023 + k) << 52)
+        mid = (decimal.Decimal(a) + decimal.Decimal(math.nextafter(a, math.inf))) / 2
+        return format(mid, 'f')
+    if c == 6:
+        # subnormals
+        x = _f64(rng.randrange(1, 1 << 52))
+        return repr(x) if rng.random() < 0.5 else '%.*e' % (rng.randint(16, 22), x)
+    if c == 7:
+        # 2^k, k = -3..70, and its neighbours
+        x = math.ldexp(1.0, rng.randint(-3, 70))
+        x = rng.choice([x, x, math.nextafter(x, 0), math.nextafter(x, math.inf)])
+        if x == int(x) and rng.random() < 0.5:
+            return str(int(x))
+        return repr(-x if rng.random() < 0.2 else x)
+    if c == 8:
+        # m * step, with its neighbouring doubles
+        s = rng.choice(SWEEP_STEPS)
+        x = float(rng.randint(-3000, 3000) * s)
+        x = rng.choice([x, x, math.nextafter(x, -math.inf),
+                        math.nextafter(x, math.inf)])
+        return str(int(x)) if x == int(x) and rng.random() < 0.5 else repr(x)
+    # the filters' constant and its neighbours
+    return repr(rng.choice([SWEEP_CONST, math.nextafter(SWEEP_CONST, 0),
+                            math.nextafter(SWEEP_CONST, math.inf), 26.0,
+                            float(TWO53)]))
+
+
+def sweep_string(rng):
+    """(the JSON text of a string body, whether it holds a \\u escape)."""
+    cps = [rng.choice(SWEEP_CPS) for _ in range(rng.randint(0, 4))]
+    if rng.random() < 0.04:
+        # escaped: the F path hands these to the general parser
+        out = []
+        for cp in cps or [0x41]:
+            if cp < 0x10000:
+                out.append('\\u%04x' % cp)
+            else:
+                v = cp - 0x10000
+                out.append('\\u%04X\\u%04X' % (0xd800 + (v >> 10),
+                                                0xdc00 + (v & 0x3ff)))
+        return ''.join(out), True
+    return ''.join(chr(cp) for cp in cps), False
+
+
+def sweep_date(rng):
+    """(a date string, its (y, mo, d, h, mi, s, ms, offset minutes) or None
+    for one that is not a date).  Only ISO forms: nothing V8's legacy parser
+    would read."""
+    y = rng.randint(0, 9999)
+    mo = rng.randint(1, 12)
+    d = rng.choice([rng.randint(1, 28), 29, 30, 31])
+    h, mi, s, ms = (rng.randint(0, 23), rng.randint(0, 59), rng.randint(0, 59),
+                    rng.randint(0, 999))
+    r = rng.random()
+    if r < 0.1:
+        h, mi, s, ms = 23, 59, 59, 999
+    elif r < 0.15:
+        h, mi, s, ms = 0, 0, 0, 0
+    ymd = '%04d-%02d-%02d' % (y, mo, d)
+    c = rng.random()
+    if c < 0.85:
+        return ymd + 'T%02d:%02d:%02d.%03dZ' % (h, mi, s, ms), \
+            (y, mo, d, h, mi, s, ms, 0)
+    if c < 0.89:
+        return ymd + 'T%02d:%02d:%02dZ' % (h, mi, s), (y, mo, d, h, mi, s, 0, 0)
+    if c < 0.93:
+        off = rng.choice([-1, 1]) * rng.randint(0, 23 * 60 + 59)
+        return ymd + 'T%02d:%02d:%02d.%03d%s%02d:%02d' % (
+            h, mi, s, ms, '-' if off < 0 else '+', abs(off) // 60,
+            abs(off) % 60), (y, mo, d, h, mi, s, ms, off)
+    if c < 0.96:
+        return ymd, (y, mo, d, 0, 0, 0, 0, 0)
+    if c < 0.98:
+        return ymd + rng.choice(['T24:00:00Z', 'T24:00:00.000Z', 'T24:00']), \
+            (y, mo, d, 24, 0, 0, 0, 0)
+    return rng.choice(['', 'x', 'never']), None
+
+
+def value_sweep_records(seed, n):
+    """n records as dicts of field -> text: num (a bare number), nstr (a
+    numeric string's body), str (a string's body), str_esc (it holds a \\u
+    escape), ts (a date string), date (ts's parts), shape (0-2)."""
+    rng = random.Random(seed)
+    out = []
+    for _ in range(n):
+        s, esc = sweep_string(rng)
+        ts, date = sweep_date(rng)
+        out.append({'num': sweep_number(rng), 'nstr': rng.choice(SWEEP_NSTR)
+                    if rng.random() < 0.7 else sweep_number(rng),
+                    'str': s, 'str_esc': esc, 'ts': ts, 'date': date,
+                    'shape': rng.randrange(3), 'len': rng.randint(130, 195)})
+    return out
+
+
+_SWEEP_SHAPES = [
+    '{"num":%(num)s,"nstr":"%(nstr)s","str":"%(str)s","ts":"%(ts)s",'
+    '"pad":"%(pad)s"}',
+    '{"ts":"%(ts)s","host":"%(pad)s","num":%(num)s,"str":"%(str)s",'
+    '"nstr":"%(nstr)s"}',
+    '{"kind":"sweep","str":"%(str)s","req":{"ts":"%(ts)s"},'
+    '"nstr":"%(nstr)s","num":%(num)s,"ts":"%(ts)s","pad":"%(pad)s"}',
+]
+
+
+def value_sweep_line(rec):
+    d = dict(rec, pad='')
+    text = _SWEEP_SHAPES[rec['shape']] % d
+    d['pad'] = 'p' * max(4, rec['len'] - len(text.encode('utf-8')))
+    return (_SWEEP_SHAPES[rec['shape']] % d).encode('utf-8')
+
+
+def value_sweep_lines(seed, n):
+    return [value_sweep_line(r) for r in value_sweep_records(seed, n)]
+
+
+def _iso_ms(ms):
+    from dragnet_b200 import jsdate
+    return jsdate.to_iso_string(ms)
+
+
+SWEEP_STR_CONSTS = ['｡', '\U0001f600']     # U+FF61 sorts above U+1F600
+
+
+def sweep_queries(records):
+    """name -> (argv, datasource properties, kind, arg) for a sweep corpus;
+    kind and arg say what sweep_reference derives (None: nothing)."""
+    q = {
+        'num': (['-b', 'num,'], None, 'discrete', None),
+        'str': (['-b', 'str,'], None, None, None),
+        'nstr': (['-b', 'nstr,'], None, None, None),
+        'num_p2': (['-b', 'num[aggr=quantize]'], None, 'p2', None),
+        'nstr_p2': (['-b', 'nstr[aggr=quantize]'], None, None, None),
+    }
+    for s in (1, 7, 100, 2147483647, 0, -3):
+        q['num_lq%d' % s] = (['-b', 'num[aggr=lquantize,step=%d]' % s],
+                             None, 'linear', s)
+    for s in (1, 3600, 86400):
+        q['ts_lq%d' % s] = (['-b', 'ts[date,field=ts,aggr=lquantize,step=%d]'
+                             % s], None, 'date', s)
+    # --after/--before on two records' seconds, and a millisecond either side
+    secs = sorted({_date_ms(r['date']) // 1000 * 1000 for r in records[:50]
+                   if r['date'] and r['date'][3] < 24})
+    lo, hi = secs[len(secs) // 4], secs[3 * len(secs) // 4]
+    for d in (-1, 0, 1):
+        q['bounds%+d' % d] = (['-b', 'nstr,', '--after', _iso_ms(lo + d),
+                               '--before', _iso_ms(hi - d)],
+                              {'timeField': 'ts'}, None, None)
+    consts = [('c', repr(SWEEP_CONST)),
+              ('c-', repr(math.nextafter(SWEEP_CONST, 0))),
+              ('c+', repr(math.nextafter(SWEEP_CONST, math.inf))),
+              ('2^53', str(TWO53)), ('"26"', '"26"')]
+    for op in ('eq', 'ne', 'lt', 'le', 'gt', 'ge'):
+        for cname, c in consts:
+            q['%s_num_%s' % (op, cname)] = (
+                ['-f', '{"%s":["num",%s]}' % (op, c), '-b', 'nstr,'], None,
+                'filter', (op, 'num', json.loads(c)))
+        # a numeric string against a number: StringToNumber, then numbers
+        q['%s_nstr_26' % op] = (['-f', '{"%s":["nstr",26]}' % op, '-b',
+                                 'nstr,'], None, None, None)
+        for i, c in enumerate(SWEEP_STR_CONSTS):
+            q['%s_str_%d' % (op, i)] = (
+                ['-f', json.dumps({op: ['str', c]}), '-b', 'str,'], None,
+                'filter', (op, 'str', c))
+    return q
+
+
+def sweep_f_decided(records, argv):
+    """How many records the F path decides itself for a sweep query: all but
+    those with an escaped string where the query reads str, and those whose
+    num is a discrete key but not a plain integer of at most 15 digits (its
+    key is Number::toString)."""
+    reads_str = any('str' in a.replace('nstr', '') for a in argv)
+    num_key = 'num,' in argv
+    n = 0
+    for r in records:
+        if reads_str and r['str_esc']:
+            continue
+        if num_key and not _simple_int(r['num']):
+            continue
+        n += 1
+    return n
+
+
+def _simple_int(t):
+    d = t[1:] if t.startswith('-') else t
+    return d.isdigit() and len(d) <= 15 and t != '-0'
+
+
+# the second reference: from the generated values, with Python's own binary64
+# (float() is correctly rounded), frexp, floor, a civil-calendar day count and
+# UTF-16 code unit order -- not the oracle's code
+
+def _days(y, m, d):
+    """Days from 1970-01-01 to y-m-d (proleptic Gregorian, any d >= 1 carries
+    into the next months)."""
+    def before_year(y):     # days from 0000-01-01 to y-01-01, y >= 0
+        return 365 * y + (y + 3) // 4 - (y + 99) // 100 + (y + 399) // 400
+    leap = y % 4 == 0 and (y % 100 != 0 or y % 400 == 0)
+    mdays = [31, 29 if leap else 28, 31, 30, 31, 30, 31, 31, 30, 31, 30, 31]
+    return before_year(y) + sum(mdays[:m - 1]) + d - 1 - before_year(1970)
+
+
+def _date_ms(p):
+    y, mo, d, h, mi, s, ms, off = p
+    return _days(y, mo, d) * 86400000 + ((h * 60 + mi) * 60 + s) * 1000 + \
+        ms - off * 60000
+
+
+def _js_string(x):
+    """Number::toString (ECMA-262 7.1.12.1) from repr's shortest digits."""
+    if x != x:
+        return 'NaN'
+    if x == 0:
+        return '0'
+    if x < 0:
+        return '-' + _js_string(-x)
+    if math.isinf(x):
+        return 'Infinity'
+    t = decimal.Decimal(repr(x)).normalize().as_tuple()
+    ds = ''.join(map(str, t.digits))
+    k, n = len(ds), t.exponent + len(ds)
+    if k <= n <= 21:
+        return ds + '0' * (n - k)
+    if 0 < n <= 21:
+        return ds[:n] + '.' + ds[n:]
+    if -6 < n <= 0:
+        return '0.' + '0' * -n + ds
+    e = '%s%d' % ('+' if n > 0 else '-', abs(n - 1))
+    return ds[0] + ('.' + ds[1:] if k > 1 else '') + 'e' + e
+
+
+def _str_value(r):
+    return json.loads('"%s"' % r['str'])
+
+
+def _ordinal_min(kind, x, step=None):
+    if kind == 'p2':
+        if x < 1:
+            return 0.0
+        if math.isinf(x):
+            return x
+        return math.ldexp(1.0, math.frexp(x)[1] - 1)
+    q = x / step
+    if math.isinf(q):
+        return q * step
+    return (math.floor(q) + 0.0) * step
+
+
+def _compare(op, a, b):
+    return {'eq': a == b, 'ne': a != b, 'lt': a < b, 'le': a <= b,
+            'gt': a > b, 'ge': a >= b}[op]
+
+
+def sweep_reference(records, kind, arg):
+    """{key: count} a sweep query must give (keys as sweep_points makes
+    them), or for lquantize with step 0 the sorted counts of its NaN
+    buckets."""
+    out = {}
+
+    def bump(k):
+        out[k] = out.get(k, 0) + 1
+    for r in records:
+        if kind == 'discrete':
+            bump(_js_string(float(r['num'])).encode())
+        elif kind == 'p2':
+            bump(_ordinal_min('p2', float(r['num'])))
+        elif kind == 'linear':
+            x = float(r['num'])
+            if arg == 0:
+                bump('+inf' if x > 0 else '-inf' if x < 0 else 'nan')
+            else:
+                bump(_ordinal_min('linear', x, arg))
+        elif kind == 'date':
+            if r['date'] is not None:
+                sec = _date_ms(r['date']) // 1000
+                bump((sec // arg) * arg + 0.0)
+        elif kind == 'filter':
+            op, field, c = arg
+            if field == 'num':
+                x, y = float(r['num']), float(c)
+                key = r['nstr'].encode()
+            else:
+                s = _str_value(r)
+                x, y = s.encode('utf-16-be'), c.encode('utf-16-be')
+                key = s.encode()
+            if _compare(op, x, y):
+                bump(key)
+    if kind == 'linear' and arg == 0:
+        return sorted(out.values())
+    return out
+
+
+def sweep_points(points, kind, arg):
+    """A scan's points in sweep_reference's form."""
+    d = {}
+    for fields, v in points:
+        x = fields[0][1]
+        k = x if isinstance(x, bytes) else ('nan' if x != x else x + 0.0)
+        d[k] = d.get(k, 0) + v
+    if kind == 'linear' and arg == 0:
+        assert set(d) <= {'nan'} and len(points) <= 3, points
+        return sorted(v for _, v in points)
+    return d

@@ -208,7 +208,7 @@ def test_medium_lines_take_the_lock_step_path(tmp_path):
     lines[100] = lines[100][:-1]                    # invalid
     lines[200] = b'{"a":"esc\\u0041","pad":"' + b'y' * 5000 + b'"}'
     path = _write(tmp_path, 'medium.log', lines)
-    for argv in (['-b', 'a'], ['-b', 'n.b.length'], []):
+    for argv in (['-b', 'a,'], ['-b', 'n.b.length'], []):
         plan = corpus.make_plan(argv)
         exp_p, exp_c = py_engine(plan, [path])
         act_p, act_c = gpu_engine(plan, [path])
@@ -223,7 +223,7 @@ def test_long_lines_and_large_counts(tmp_path):
              b'{"pad":"' + b'q' * 200000 + b'","a":"t"}'] + [b'{"a":1}'] * 50000
     lines += [b''] * 30000 + [b'{"a":"s"}']
     path = _write(tmp_path, 'long.log', lines)
-    plan = corpus.make_plan(['-b', 'a'])
+    plan = corpus.make_plan(['-b', 'a,'])
     exp_p, exp_c = py_engine(plan, [path])
     act_p, act_c = gpu_engine(plan, [path])
     assert canon_points(act_p) == canon_points(exp_p)
@@ -306,8 +306,8 @@ def test_scalar_forms_behind_one_template(pad, tmp_path):
         pytest.skip('lines of 16 bytes: the F kernel hands them all over')
     jit_expected = os.environ.get('DNG_JIT') == 'sync'
     path = _write(tmp_path, 'scalars.log', lines)
-    for argv in (['-b', 'a'], ['-b', 's'], ['-b', 'a[aggr=quantize]'],
-                 ['-b', 'a,s', '-f', '{"ge":["a",1]}']):
+    for argv in (['-b', 'a,'], ['-b', 's,'], ['-b', 'a[aggr=quantize]'],
+                 ['-b', 'a,s,', '-f', '{"ge":["a",1]}']):
         plan = corpus.make_plan(argv)
         exp_p, exp_c = py_engine(plan, [path])
         r = datasource_gpu.run_plan(plan, files=[path])
@@ -356,7 +356,7 @@ def test_stream_that_changes_shape_is_relearned(tmp_path):
                  (i % 7, i % 3, i % 17) for i in range(1200000))
     path = tmp_path / 'two.log'
     path.write_bytes(a + b)
-    plan = corpus.make_plan(['-b', 'a,n'])
+    plan = corpus.make_plan(['-b', 'a,n,'])
     exp_p, exp_c = cpp_engine(plan, [str(path)], threads=8)
     r = datasource_gpu.run_plan(plan, chunks=_chunks(a + b, 4 << 20))
     assert canon_points(r.points) == canon_points(exp_p)
@@ -376,7 +376,7 @@ def test_stream_that_turns_to_long_lines_switches_kernel(tmp_path):
                  b'","n":%d}\n' % (i % 7) for i in range(12000))
     path = tmp_path / 'long.log'
     path.write_bytes(a + b)
-    plan = corpus.make_plan(['-b', 'a,n'])
+    plan = corpus.make_plan(['-b', 'a,n,'])
     exp_p, exp_c = cpp_engine(plan, [str(path)], threads=8)
     r = datasource_gpu.run_plan(plan, chunks=_chunks(a + b, 4 << 20))
     assert canon_points(r.points) == canon_points(exp_p)
@@ -406,7 +406,7 @@ def test_optional_fields_make_a_branching_trie(tmp_path):
         parts.append(b'"z":"end"')
         lines.append(b'{' + b','.join(parts) + b'}')
     path = _write(tmp_path, 'opt.log', lines)
-    plan = corpus.make_plan(['-b', 'a,b.c,d'])
+    plan = corpus.make_plan(['-b', 'a,b.c,d,'])
     exp_p, exp_c = cpp_engine(plan, [path], threads=4)
     r = datasource_gpu.run_plan(plan, files=[path])
     assert canon_points(r.points) == canon_points(exp_p)

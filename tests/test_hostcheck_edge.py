@@ -85,8 +85,8 @@ def test_scalar_forms_behind_one_template(tmp_path):
     wildcard scans."""
     lines = [b'{"a":7,"s":"k0"}'] * 3 + corpus.scalar_lines()
     path = _write(tmp_path, 'scalars.log', lines)
-    for argv in (['-b', 'a'], ['-b', 's'], ['-b', 'a[aggr=quantize]'],
-                 ['-b', 'a,s', '-f', '{"ge":["a",1]}']):
+    for argv in (['-b', 'a,'], ['-b', 's,'], ['-b', 'a[aggr=quantize]'],
+                 ['-b', 'a,s,', '-f', '{"ge":["a",1]}']):
         _compare(corpus.make_plan(argv), path)
 
 

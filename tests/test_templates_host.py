@@ -57,7 +57,7 @@ def test_shapes_that_cannot_be_templates_fall_through(tmp_path):
     # the array shape needs index semantics: never templated
     assert doc['ntmpl'] == 40, (doc['ntmpl'], dbg)
     assert doc['counters']['invalid_json'] == 5
-    doc, dbg = run_tmpl(corpus.make_plan(['-b', 'a,n']), str(p), tmp_path)
+    doc, dbg = run_tmpl(corpus.make_plan(['-b', 'a,n,']), str(p), tmp_path)
     assert doc['ntmpl'] == 80, (doc['ntmpl'], dbg)
 
 
@@ -83,7 +83,7 @@ def test_optional_fields_make_a_branching_trie(tmp_path):
         lines.append(b'{' + b','.join(parts) + b'}')
     p = tmp_path / 'opt.log'
     p.write_bytes(b'\n'.join(lines) + b'\n')
-    plan = corpus.make_plan(['-b', 'a,b.c,d'])
+    plan = corpus.make_plan(['-b', 'a,b.c,d,'])
     doc, dbg = run_tmpl(plan, str(p), tmp_path)
     assert doc['ntmpl'] == len(lines), (doc['ntmpl'], dbg)
     assert '16 leaves' in dbg, dbg
