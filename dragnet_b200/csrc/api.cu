@@ -1583,6 +1583,11 @@ int dng_scan_tally_stats(dng_scan *s, uint64_t *inline_overflow, int *f_warps)
 	return DNG_OK;
 }
 
+void dng_jit_finish(void)
+{
+	dng::jit_finish();
+}
+
 void dng_release_cached(void)
 {
 	BufCache &c = buf_cache();

@@ -669,11 +669,116 @@ double now_ms()
 	    std::chrono::steady_clock::now().time_since_epoch()).count();
 }
 
+/* one build at a time: two links running side by side (scans started in quick
+ * succession, each with its compiler thread) have crashed inside libnvJitLink */
+std::mutex build_mu;
+
+/* CUDA source -> LTO-IR, within the register budget of the kernel it becomes
+ * part of (__launch_bounds__(F_NT = 896, 1): 72 registers) */
+bool compile_ltoir(Libs &L, const std::string &source, std::string &ir,
+    std::string &err)
+{
+	nvrtcProgram prog = nullptr;
+	if (L.CreateProgram(&prog, source.c_str(), "dng_jmatch.cu", 0, nullptr,
+	    nullptr) != 0) {
+		err = "nvrtcCreateProgram failed";
+		return false;
+	}
+	const char *opts[] = { "-arch=sm_90a", "-rdc=true", "-dlto",
+	    "-maxrregcount=72", "-std=c++17", "-lineinfo" };
+	const int rc = L.CompileProgram(prog, 6, opts);
+	if (rc != 0) {
+		size_t n = 0;
+		L.GetProgramLogSize(prog, &n);
+		std::string log(n, '\0');
+		if (n)
+			L.GetProgramLog(prog, &log[0]);
+		err = "nvrtcCompileProgram: " + log;
+		L.DestroyProgram(&prog);
+		return false;
+	}
+	size_t n = 0;
+	L.GetLTOIRSize(prog, &n);
+	ir.assign(n, '\0');
+	L.GetLTOIR(prog, &ir[0]);
+	L.DestroyProgram(&prog);
+	return true;
+}
+
+struct LinkInput {
+	int kind;		/* nvJitLinkInputType */
+	const void *data;
+	size_t size;
+	const char *name;
+};
+enum { IN_CUBIN = 1, IN_LTOIR = 3, IN_FATBIN = 4 };
+
+bool link_cubin(Libs &L, const LinkInput *in, int nin, std::string &cubin,
+    std::string &err)
+{
+	nvJitLinkHandle h = nullptr;
+	const char *lopts[] = { "-arch=sm_90a", "-lto", "-maxrregcount=72",
+	    "-lineinfo" };
+	if (L.LCreate(&h, 4, lopts) != 0) {
+		err = "nvJitLinkCreate failed";
+		return false;
+	}
+	int lrc = 0;
+	for (int i = 0; i < nin && lrc == 0; i++)
+		lrc = L.LAddData(h, in[i].kind, in[i].data, in[i].size,
+		    in[i].name);
+	if (lrc == 0)
+		lrc = L.LComplete(h);
+	if (lrc != 0) {
+		size_t en = 0;
+		L.LErrSize(h, &en);
+		std::string log(en, '\0');
+		if (en)
+			L.LErr(h, &log[0]);
+		err = "nvJitLink: " + log;
+		L.LDestroy(&h);
+		return false;
+	}
+	size_t cn = 0;
+	L.LCubinSize(h, &cn);
+	cubin.assign(cn, '\0');
+	L.LCubin(h, &cubin[0]);
+	L.LDestroy(&h);
+	return true;
+}
+
 } /* namespace */
 
 bool jit_prepare()
 {
-	return libs().ok;
+	Libs &L = libs();
+	if (!L.ok)
+		return false;
+	/*
+	 * Both libraries register exit-time destructors on first use, from
+	 * inside the first compile and the first link -- later than anything
+	 * registered before that build started.  exit() runs such handlers in
+	 * the reverse order of registration, so with a build in flight on a
+	 * worker thread their teardown ran BEFORE the handler that joins the
+	 * worker (jit_load.cpp), under the build: a segfault or a hang after
+	 * everything else had finished.  A first compile and link of an empty
+	 * kernel, here on the caller's thread, gets most of those registrations
+	 * done before the caller registers its handler (libnvJitLink still
+	 * makes some in its first real link: dng_jit_finish() is what makes
+	 * exit safe).
+	 */
+	static std::once_flag once;
+	std::call_once(once, [&L] {
+		std::lock_guard<std::mutex> build_lock(build_mu);
+		std::string ir, cubin, err;
+		if (compile_ltoir(L, "extern \"C\" __global__ void "
+		    "dng_jit_warm_up() {}\n", ir, err)) {
+			const LinkInput in = { IN_LTOIR, ir.data(), ir.size(),
+			    "dng_jit_warm_up" };
+			link_cubin(L, &in, 1, cubin, err);
+		}
+	});
+	return true;
 }
 
 bool jit_build(const std::string &source, int nsl, std::string &cubin,
@@ -694,74 +799,22 @@ bool jit_build(const std::string &source, int nsl, std::string &cubin,
 		err = "no kernel for this slice size";
 		return false;
 	}
-	/* one build at a time: two links running side by side (scans started in
-	 * quick succession, each with its compiler thread) have crashed inside
-	 * libnvJitLink */
-	static std::mutex build_mu;
 	std::lock_guard<std::mutex> build_lock(build_mu);
 	const double t0 = now_ms();
-	nvrtcProgram prog = nullptr;
-	if (L.CreateProgram(&prog, source.c_str(), "dng_jmatch.cu", 0, nullptr,
-	    nullptr) != 0) {
-		err = "nvrtcCreateProgram failed";
+	std::string ir;
+	if (!compile_ltoir(L, source, ir, err))
 		return false;
-	}
-	/* LTO-IR, within the register budget of the kernel it becomes part of
-	 * (__launch_bounds__(F_NT = 896, 1): 72 registers) */
-	const char *opts[] = { "-arch=sm_90a", "-rdc=true", "-dlto",
-	    "-maxrregcount=72", "-std=c++17", "-lineinfo" };
-	const int rc = L.CompileProgram(prog, 6, opts);
-	if (rc != 0) {
-		size_t n = 0;
-		L.GetProgramLogSize(prog, &n);
-		std::string log(n, '\0');
-		if (n)
-			L.GetProgramLog(prog, &log[0]);
-		err = "nvrtcCompileProgram: " + log;
-		L.DestroyProgram(&prog);
-		return false;
-	}
-	size_t n = 0;
-	L.GetLTOIRSize(prog, &n);
-	std::string ir(n, '\0');
-	L.GetLTOIR(prog, &ir[0]);
-	L.DestroyProgram(&prog);
 	const double t1 = now_ms();
 	if (compile_ms)
 		*compile_ms = t1 - t0;
-
-	nvJitLinkHandle h = nullptr;
-	const char *lopts[] = { "-arch=sm_90a", "-lto", "-maxrregcount=72",
-	    "-lineinfo" };
-	if (L.LCreate(&h, 4, lopts) != 0) {
-		err = "nvJitLinkCreate failed";
+	const LinkInput in[] = {
+		{ IN_FATBIN, hot, (size_t)(hot_end - hot), "fast_jit" },
+		{ IN_LTOIR, ir.data(), ir.size(), "dng_jmatch" },
+		{ IN_CUBIN, dng_jit_cold, (size_t)(dng_jit_cold_end -
+		    dng_jit_cold), "fast_jit_cold" },
+	};
+	if (!link_cubin(L, in, 3, cubin, err))
 		return false;
-	}
-	const int IN_CUBIN = 1, IN_LTOIR = 3, IN_FATBIN = 4;
-	int lrc = L.LAddData(h, IN_FATBIN, hot, (size_t)(hot_end - hot),
-	    "fast_jit");
-	if (lrc == 0)
-		lrc = L.LAddData(h, IN_LTOIR, ir.data(), ir.size(), "dng_jmatch");
-	if (lrc == 0)
-		lrc = L.LAddData(h, IN_CUBIN, dng_jit_cold,
-		    (size_t)(dng_jit_cold_end - dng_jit_cold), "fast_jit_cold");
-	if (lrc == 0)
-		lrc = L.LComplete(h);
-	if (lrc != 0) {
-		size_t en = 0;
-		L.LErrSize(h, &en);
-		std::string log(en, '\0');
-		if (en)
-			L.LErr(h, &log[0]);
-		err = "nvJitLink: " + log;
-		L.LDestroy(&h);
-		return false;
-	}
-	size_t cn = 0;
-	L.LCubinSize(h, &cn);
-	cubin.assign(cn, '\0');
-	L.LCubin(h, &cubin[0]);
-	L.LDestroy(&h);
 	if (link_ms)
 		*link_ms = now_ms() - t1;
 	return true;

@@ -58,8 +58,13 @@ std::shared_ptr<JitKernels> jit_request(const std::string &source, int nsl,
     int dev, int smem_max, bool wait);
 
 /* load the two compiler libraries now, on this thread (they are dlopen()ed
- * once per process); false if they are not there */
+ * once per process), and compile and link an empty kernel with them once, so
+ * that the exit handlers they register on first use are registered before any
+ * the caller registers next; false if they are not there */
 bool jit_prepare();
+
+/* dng_jit_finish(): join the compiler threads, drop queued builds */
+void jit_finish();
 
 /* only compile + link, to `cubin` (no device needed: tests); nsl = 16-byte
  * units per lane slice: 7, 9, 11 or 13 */

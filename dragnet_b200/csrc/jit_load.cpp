@@ -22,11 +22,14 @@ std::condition_variable g_cv;
 std::map<std::pair<int, u64>, std::shared_ptr<JitKernels>> g_cache;
 
 /*
- * Compiler threads are joined before the process goes away: by an atexit()
- * handler registered once the compiler libraries are loaded -- so that it runs
- * BEFORE their own exit handlers and static destructors (a compile in flight
- * while libnvrtc tears itself down ends in free(): invalid pointer) -- and, for
- * good measure, when this library's statics go.
+ * Compiler threads must be joined before the compiler libraries tear
+ * themselves down at exit (a compile in flight while they do segfaults or
+ * hangs): by dng_jit_finish(), which the host calls before it exits (the
+ * Python package from atexit); failing that, by an atexit() handler
+ * registered after jit_prepare() -- which loads the libraries and runs them
+ * once, so that most of the exit handlers they register come before it and
+ * run after it (not all: libnvJitLink registers some only in its first real
+ * link) -- and, for good measure, when this library's statics go.
  */
 struct Workers {
 	std::vector<std::thread> th;
@@ -106,6 +109,11 @@ void build_into(std::shared_ptr<JitKernels> k, std::string source, int nsl,
 
 } /* namespace */
 
+void jit_finish()
+{
+	join_workers_at_exit();
+}
+
 std::shared_ptr<JitKernels> jit_request(const std::string &source, int nsl,
     int dev, int smem_max, bool wait)
 {
@@ -129,8 +137,8 @@ std::shared_ptr<JitKernels> jit_request(const std::string &source, int nsl,
 			build_into(k, source, nsl, dev, smem_max, key);
 			g.lock();
 		} else {
-			/* (the libraries first, here, and then the handler that
-			 * waits for the thread: see Workers) */
+			/* (the libraries loaded and run once, here, and then
+			 * the handler that waits for the thread: see Workers) */
 			g.unlock();
 			jit_prepare();
 			static std::once_flag once;

@@ -5,6 +5,7 @@ This is the Python stand-in for the N-API addon a Node deployment would use
 loudly when the library has not been built; there is no fallback.
 """
 
+import atexit
 import ctypes
 import os
 
@@ -70,6 +71,7 @@ _SIGS = [
     ('dng_scan_error', ctypes.c_char_p, [_P]),
     ('dng_scan_destroy', None, [_P]),
     ('dng_release_cached', None, []),
+    ('dng_jit_finish', None, []),
     ('dng_scan_kernel_stats', ctypes.c_int,
      [_P, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_uint64),
       ctypes.POINTER(ctypes.c_uint64)]),
@@ -150,6 +152,10 @@ def lib():
             fn.restype = res
             fn.argtypes = args
         _lib = L
+        # before the interpreter's own teardown and the C exit handlers:
+        # a background compile still running when the compiler libraries
+        # tear themselves down at exit() can crash the process
+        atexit.register(L.dng_jit_finish)
     return _lib
 
 

@@ -143,6 +143,12 @@ void dng_scan_destroy(dng_scan *scan);
  * this process (bounded by DNG_CACHE_BYTES per kind, default 2 GiB); this
  * returns them to the driver. */
 void dng_release_cached(void);
+/* Waits for the matchers being compiled in the background (DNG_JIT=async,
+ * the default) and drops those still queued; later scans compile none in the
+ * background.  Call it before the process exits: a compile still running when
+ * exit() tears the compiler libraries down can crash the process.  The Python
+ * package calls it from an atexit handler. */
+void dng_jit_finish(void);
 
 /* Device time (ms, CUDA events on the scan stream) spent in scan kernels and
  * the number of kernel launches since open; for bench.py's roofline. */

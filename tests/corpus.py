@@ -1045,3 +1045,551 @@ def sweep_points(points, kind, arg):
         assert set(d) <= {'nan'} and len(points) <= 3, points
         return sorted(v for _, v in points)
     return d
+
+
+# ---------------------------------------------------------------------------
+# krill filters: records whose `v` takes every value form a JSON field can
+# have, the constants a filter compares it with, seeded predicate trees, and a
+# second reference for them written from ECMA-262 (not the oracle's code)
+# ---------------------------------------------------------------------------
+
+MISSING = object()      # a field the record does not have
+
+# (tag, JSON text, value as krill_reference sees it) of every form `v` takes;
+# numbers are floats, strings str, containers dict / list
+V_FORMS = [
+    ('missing', None, MISSING),
+    ('null', 'null', None), ('true', 'true', True), ('false', 'false', False),
+    ('zero', '0', 0.0), ('negzero', '-0', -0.0), ('int', None, None),
+    ('tenth', '0.1', 0.1), ('e21', '1e21', 1e21),
+    ('two53p1', '9007199254740993', float(TWO53)),
+    ('s_empty', '""', ''), ('s_0', '"0"', '0'), ('s_26', '"26"', '26'),
+    ('s_sp26', '" 26 "', ' 26 '), ('s_hex', '"0x1a"', '0x1a'),
+    ('s_abc', '"abc"', 'abc'), ('s_get', '"GET"', 'GET'),
+    ('s_kana', '"ｶﾀ"', 'ｶﾀ'),
+    ('s_emoji', '"\U0001f600"', '\U0001f600'),
+    ('s_quote', '"x\\"y"', 'x"y'), ('s_escA', '"\\u0041"', 'A'),
+    ('obj', '{}', {}), ('arr', '[1,2]', [1.0, 2.0]), ('arr0', '[]', []),
+]
+V_INTS = [1, 2, 25, 26, 27, -1, 100]
+
+# the constants of the filters: numbers around the forms above, strings
+# equal to some of them, a prefix of none, and the two booleans
+KRILL_CONSTS = [0, -0.0, 1, 26, 0.1, TWO53, 1e21, '', '0', '26', ' 26 ',
+                '0x1a', 'abc', 'GET', 'x"y', 'A', 'ｶﾀ', True, False]
+
+S_VALUES = ['GET', 'GEX', 'G', 'GF', 'GETS', 'GETSA', 'GETSAB', 'GETSABC',
+            'GETSABCD', 'PUT', 'abc', '26', '', ' 26 ', '0x1a']
+OPT_VALUES = [('0', 0.0), ('26', 26.0), ('"26"', '26'), ('"abc"', 'abc'),
+              ('true', True), ('null', None)]
+
+# field orders of the four record shapes; only shapes 0 and 2 have `opt`,
+# shape 3 has a literal key "a.b" (pluck reads it before a.b)
+_FILTER_SHAPES = [
+    ['tag', 'v', 'n', 's', 'b', 'opt', 'a', 't', 'pad'],
+    ['t', 'tag', 'a', 'n', 'v', 's', 'b', 'pad'],
+    ['tag', 's', 'v', 'opt', 'b', 'n', 't', 'a', 'pad'],
+    ['tag', 'a.b', 'v', 'n', 'a', 's', 'b', 't', 'pad'],
+]
+FILTER_DAY_MS = 1398902400000       # 2014-05-01T00:00:00.000Z
+
+
+def filter_records(seed, n):
+    """n records as dicts: tag, v_text/v (the form of `v`), n, s, b, opt
+    (MISSING in shapes 1 and 3), ab (what pluck(rec, "a.b") gives), t_ms,
+    shape, len (the line's length in bytes) and damage (None, 'cut' or a
+    junk suffix)."""
+    rng = random.Random(seed)
+    out = []
+    for _ in range(n):
+        tag, text, val = rng.choice(V_FORMS)
+        if tag == 'int':
+            k = rng.choice(V_INTS)
+            text, val = str(k), float(k)
+        shape = rng.randrange(4)
+        nv = rng.choice([rng.randint(-5, 300), 26, 0])
+        ot, ov = rng.choice(OPT_VALUES)
+        ab = rng.randint(0, 40)
+        r = rng.random()
+        damage = 'cut' if r < 0.005 else \
+            rng.choice(['x', ',', '}', ' 1', '{}']) if r < 0.01 else None
+        out.append({'tag': tag, 'v_text': text, 'v': val,
+                    'n': float(nv), 'n_text': str(nv),
+                    's': rng.choice(S_VALUES), 'b': rng.random() < 0.5,
+                    'opt_text': ot if shape in (0, 2) else None,
+                    'opt': ov if shape in (0, 2) else MISSING,
+                    'ab': float(ab), 'ab2': ab + 1,
+                    't_ms': FILTER_DAY_MS + rng.randrange(86400000),
+                    'shape': shape, 'len': rng.randint(120, 215),
+                    'damage': damage})
+    return out
+
+
+def _iso_z(ms):
+    s, ms = divmod(ms - FILTER_DAY_MS, 1000)
+    return '2014-05-01T%02d:%02d:%02d.%03dZ' % (s // 3600, s // 60 % 60,
+                                                 s % 60, ms)
+
+
+def filter_line(rec):
+    def render(pad):
+        parts = []
+        for f in _FILTER_SHAPES[rec['shape']]:
+            if f == 'tag':
+                parts.append('"tag":"%s"' % rec['tag'])
+            elif f == 'v' and rec['v'] is not MISSING:
+                parts.append('"v":' + rec['v_text'])
+            elif f == 'n':
+                parts.append('"n":' + rec['n_text'])
+            elif f == 's':
+                parts.append('"s":' + json.dumps(rec['s']))
+            elif f == 'b':
+                parts.append('"b":' + ('true' if rec['b'] else 'false'))
+            elif f == 'opt' and rec['opt'] is not MISSING:
+                parts.append('"opt":' + rec['opt_text'])
+            elif f == 'a':
+                parts.append('"a":{"b":%d}' % (rec['ab2'] if rec['shape'] == 3
+                                               else int(rec['ab'])))
+            elif f == 'a.b':
+                parts.append('"a.b":%d' % int(rec['ab']))
+            elif f == 't':
+                parts.append('"t":"%s"' % _iso_z(rec['t_ms']))
+            elif f == 'pad':
+                parts.append('"pad":"%s"' % pad)
+        return ('{' + ','.join(parts) + '}').encode('utf-8')
+    line = render('')
+    line = render('p' * max(8, rec['len'] - len(line)))
+    if rec['damage'] == 'cut':          # after every field a filter reads
+        return line[:-4]
+    if rec['damage']:
+        return line + rec['damage'].encode()
+    return line
+
+
+def filter_lines(seed, n):
+    return [filter_line(r) for r in filter_records(seed, n)]
+
+
+FILTER_FIELDS = ['v', 'v', 'v', 'n', 's', 'b', 'opt', 'a.b', 'nope']
+OPS = ['eq', 'ne', 'lt', 'le', 'gt', 'ge']
+
+
+def random_predicate(rng, nleaves, fields=FILTER_FIELDS, depth=0):
+    """A krill tree of `nleaves` leaves (counting each `{}` child, which
+    compiles to a leaf too): and/or nodes of 1-5 children nested at most 5
+    deep, leaves of every operator over `fields` with constants of
+    KRILL_CONSTS."""
+    if nleaves == 1:
+        if depth and rng.random() < 0.08:
+            return {}
+        return {rng.choice(OPS): [rng.choice(fields),
+                                  rng.choice(KRILL_CONSTS)]}
+    cap = 5 ** (4 - depth)          # leaves a child at depth + 1 can hold
+    lo = max(1, -(-nleaves // cap))
+    k = rng.randint(lo, max(lo, min(5, nleaves)))
+    # nleaves split into k parts, each 1..cap
+    parts = [1] * k
+    for _ in range(nleaves - k):
+        i = rng.choice([j for j in range(k) if parts[j] < cap])
+        parts[i] += 1
+    return {rng.choice(['and', 'or']): [
+        random_predicate(rng, p, fields, depth + 1) for p in parts]}
+
+
+def predicate_leaves(pred):
+    """Leaves the plan compiler emits for pred ({} children count)."""
+    if not pred:
+        return 1
+    key = next(iter(pred))
+    if key in ('and', 'or'):
+        return sum(predicate_leaves(p) for p in pred[key])
+    return 1
+
+
+# --- the second reference: ECMA-262 7.2.13 / 7.2.14 on the values above ---
+
+# WhiteSpace and LineTerminator (ECMA-262 12.2, 12.3)
+_JS_WS = ('\t\n\v\f\r \u00a0\u1680\u2000\u2001\u2002\u2003\u2004'
+          '\u2005\u2006\u2007\u2008\u2009\u200a\u2028\u2029\u202f'
+          '\u205f\u3000\ufeff')
+
+
+class FieldMissing(Exception):
+    pass
+
+
+def _js_type(x):
+    if x is None:
+        return 'null'
+    if isinstance(x, bool):
+        return 'boolean'
+    if isinstance(x, float):
+        return 'number'
+    if isinstance(x, str):
+        return 'string'
+    return 'object'
+
+
+def _string_to_number(s):
+    """StringToNumber (ECMA-262 7.1.4.1.1)."""
+    s = s.strip(_JS_WS)
+    if s == '':
+        return 0.0
+    for pre, base, digits in (('0x', 16, '0123456789abcdef'),
+                              ('0o', 8, '01234567'), ('0b', 2, '01')):
+        if s[:2].lower() == pre:
+            body = s[2:]
+            if body and all(c in digits for c in body.lower()):
+                return float(int(body, base))
+            return math.nan
+    sign, body = 1.0, s
+    if body[:1] in '+-':
+        sign, body = (-1.0 if body[0] == '-' else 1.0), body[1:]
+    if body == 'Infinity':
+        return sign * math.inf
+    mant, _, exp = body.partition('e') if 'e' in body else \
+        body.partition('E')
+    if exp[:1] in '+-':
+        exp = exp[1:]
+    if ('e' in body or 'E' in body) and not (exp and exp.isdigit()):
+        return math.nan
+    ip, dot, fp = mant.partition('.')
+    if not (ip or fp) or not all(c.isdigit() and c.isascii()
+                                 for c in ip + fp):
+        return math.nan
+    return sign * float(body)
+
+
+def _to_primitive(x):
+    """ToPrimitive(x, hint number) of a JSON value: objects give
+    "[object Object]", arrays Array.prototype.join."""
+    if isinstance(x, dict):
+        return '[object Object]'
+    if isinstance(x, list):
+        return ','.join('' if e is None else _to_string(e) for e in x)
+    return x
+
+
+def _to_string(x):
+    if isinstance(x, float):
+        return _js_string(x)
+    if isinstance(x, bool):
+        return 'true' if x else 'false'
+    if x is None:
+        return 'null'
+    if isinstance(x, str):
+        return x
+    return _to_primitive(x)
+
+
+def _to_number(x):
+    x = _to_primitive(x)
+    if x is None:
+        return 0.0
+    if isinstance(x, bool):
+        return 1.0 if x else 0.0
+    if isinstance(x, str):
+        return _string_to_number(x)
+    return x
+
+
+def loose_equals(x, y):
+    """x == y (IsLooselyEqual, ECMA-262 7.2.14)."""
+    tx, ty = _js_type(x), _js_type(y)
+    if tx == ty:
+        return x is y if tx == 'object' else x == y
+    if 'null' in (tx, ty):
+        return False            # (no undefined here: it raised before)
+    if tx == 'number' and ty == 'string':
+        return x == _string_to_number(y)
+    if tx == 'string' and ty == 'number':
+        return _string_to_number(x) == y
+    if tx == 'boolean':
+        return loose_equals(1.0 if x else 0.0, y)
+    if ty == 'boolean':
+        return loose_equals(x, 1.0 if y else 0.0)
+    if tx == 'object':
+        return loose_equals(_to_primitive(x), y)
+    return False
+
+
+def _less_than(x, y):
+    """IsLessThan (ECMA-262 7.2.13): True, False or None (undefined)."""
+    px, py = _to_primitive(x), _to_primitive(y)
+    if isinstance(px, str) and isinstance(py, str):
+        # UTF-16 code units: big-endian UTF-16 bytes order the same way
+        return px.encode('utf-16-be') < py.encode('utf-16-be')
+    nx, ny = _to_number(px), _to_number(py)
+    if nx != nx or ny != ny:
+        return None
+    return nx < ny
+
+
+def js_compare(op, x, y):
+    if op == 'eq':
+        return loose_equals(x, y)
+    if op == 'ne':
+        return not loose_equals(x, y)
+    if op == 'lt':
+        return _less_than(x, y) is True
+    if op == 'gt':
+        return _less_than(y, x) is True
+    if op == 'le':
+        return _less_than(y, x) is False
+    return _less_than(x, y) is False
+
+
+def _field(rec, name):
+    v = {'v': rec['v'], 'n': rec['n'], 's': rec['s'], 'b': rec['b'],
+         'opt': rec['opt'], 'a.b': rec['ab'], 'tag': rec['tag']}.get(
+             name, MISSING)
+    if v is MISSING:
+        raise FieldMissing(name)
+    return v
+
+
+def krill_test(pred, rec):
+    """krill's evaluation of pred on rec: left to right, short-circuit; a
+    leaf on a field the record does not have raises FieldMissing."""
+    if not pred:
+        return True
+    key = next(iter(pred))
+    if key == 'and':
+        return all(krill_test(p, rec) for p in pred[key])
+    if key == 'or':
+        return any(krill_test(p, rec) for p in pred[key])
+    field, c = pred[key]
+    if isinstance(c, int) and not isinstance(c, bool):
+        c = float(c)
+    return js_compare(key, _field(rec, field), c)
+
+
+def krill_reference(records, pred, ds=None, bounds=None):
+    """What `-f pred -b tag,` over records gives, with an optional
+    datasource filter ds and time bounds (ge_ms, lt_ms) on t:
+    ({tag: count}, {stage: (noutputs, nfilteredout, nfailedeval)})."""
+    tally = {}
+    stages = [(name, p) for name, p in (('Datasource filter', ds),
+                                        ('User filter', pred)) if p]
+    split = {name: [0, 0, 0] for name, _ in stages}
+    if bounds:
+        split['Time filter'] = [0, 0, 0]
+    for r in records:
+        if r['damage']:
+            continue
+        passed = True
+        for name, p in stages:
+            try:
+                ok = krill_test(p, r)
+            except FieldMissing:
+                split[name][2] += 1
+                passed = False
+                break
+            if not ok:
+                split[name][1] += 1
+                passed = False
+                break
+            split[name][0] += 1
+        if passed and bounds:
+            if not bounds[0] <= r['t_ms'] < bounds[1]:
+                split['Time filter'][1] += 1
+                passed = False
+            else:
+                split['Time filter'][0] += 1
+        if passed:
+            tally[r['tag'].encode()] = tally.get(r['tag'].encode(), 0) + 1
+    return tally, {k: tuple(v) for k, v in split.items()}
+
+
+def filter_split(counters, stage):
+    """(noutputs, nfilteredout, nfailedeval) of a stage of a scan's
+    counters."""
+    c = counters.get(stage, {})
+    return (c.get('noutputs', 0), c.get('nfilteredout', 0),
+            c.get('nfailedeval', 0))
+
+
+def tag_points(points):
+    """{tag: count} of the points of a `-b tag,` scan."""
+    out = {}
+    for fields, v in points:
+        out[fields[0][1]] = out.get(fields[0][1], 0) + v
+    return out
+
+
+# --- the queries of the filter tests ---
+
+FILTER_AFTER, FILTER_BEFORE = '2014-05-01T06:00:00.000Z', \
+    '2014-05-01T18:30:00.000Z'
+FILTER_BOUNDS = (FILTER_DAY_MS + 6 * 3600000,
+                 FILTER_DAY_MS + 18 * 3600000 + 1800000)
+# sizes of the random trees: every size up to the plan's 48 leaves, most
+# around the F path's 16
+TREE_SIZES = [1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11, 12, 13] + \
+    list(range(14, 19)) * 4 + [19, 20, 21, 22, 23, 24, 25, 26, 27, 28, 30,
+                               32, 33, 35, 36, 38, 40, 42, 44, 45, 46, 47,
+                               48]
+
+
+def filter_queries():
+    """name -> (argv, datasource properties, user predicate, datasource
+    predicate, time bounds) of every filter query: the comparison matrix
+    (op_<const>), the random trees (tree<i>_<leaves>: the odd ones read only
+    v and opt, so that with tag they need three capture rows) and the
+    combined programs (comb16, comb17: leaves of the datasource filter, the
+    user filter and the two time-bound leaves together)."""
+    q = {}
+    for op in OPS:
+        for c in KRILL_CONSTS:
+            pred = {op: ['v', c]}
+            q['%s_%s' % (op, json.dumps(c, ensure_ascii=False))] = (
+                ['-f', json.dumps(pred), '-b', 'tag,'], None, pred, None,
+                None)
+    rng = random.Random(4242)
+    for i, n in enumerate(TREE_SIZES):
+        pred = random_predicate(rng, n, FILTER_FIELDS if i % 2 == 0 else
+                                ('v', 'v', 'opt'))
+        q['tree%02d_%d' % (i, n)] = (['-f', json.dumps(pred), '-b', 'tag,'],
+                                     None, pred, None, None)
+    for total in (16, 17):
+        ds = random_predicate(rng, 6, ('v',))
+        pred = random_predicate(rng, total - 8, ('v',))
+        q['comb%d' % total] = (
+            ['-f', json.dumps(pred), '-b', 'tag,', '--after', FILTER_AFTER,
+             '--before', FILTER_BEFORE], {'filter': ds, 'timeField': 't'},
+            pred, ds, FILTER_BOUNDS)
+    return q
+
+
+def filter_jit_names(names):
+    """The filter queries a run-time compiled F kernel is built for (each
+    distinct plan costs a link): one constant of each type per operator,
+    the trees of 14-18 leaves and the combined programs."""
+    return sorted(
+        [n for n in names if n.split('_', 1)[0] in OPS and
+         n.split('_', 1)[1] in ('26', '"26"', 'true')] +
+        [n for n in names if n.startswith('tree') and
+         14 <= int(n.rsplit('_', 1)[1]) <= 18] +
+        [n for n in names if n.startswith('comb')])
+
+
+def query_leaves(query):
+    """Leaves of a filter query's whole plan."""
+    _, _, pred, ds, bounds = query
+    return (predicate_leaves(pred) if pred else 0) + \
+        (predicate_leaves(ds) if ds else 0) + (2 if bounds else 0)
+
+
+def _pred_fields(pred):
+    if not pred:
+        return set()
+    key = next(iter(pred))
+    if key in ('and', 'or'):
+        return set().union(*(_pred_fields(p) for p in pred[key]))
+    return {pred[key][0]}
+
+
+def query_capture_rows(query):
+    """Capture rows the F kernel needs for a filter query (fast.cpp
+    fplan_build): one per distinct field, here the filters' fields, tag and
+    the time field; its only column, tag, is not bucketized."""
+    _, _, pred, ds, bounds = query
+    return len(_pred_fields(pred) | _pred_fields(ds) | {'tag'} |
+               ({'t'} if bounds else set()))
+
+
+def _or_eq(fields_consts):
+    return json.dumps({'or': [{'eq': [f, c]} for f, c in fields_consts]})
+
+
+# the plan compiler's limits (plan.cpp), each as (argv at the limit, argv one
+# past it, the DNG_ELIMIT message of the second)
+_COMPONENTS_30 = ['a.b.c.d.e.f.g.h', 'a.b.c.d.e.f.g.i', 'a.b.c.d.e.f.g.j',
+                  'a.b.c.x']          # + tag + v: 30 path components
+PLAN_LIMITS = {
+    'leaves_48': (
+        ['-f', json.dumps(random_predicate(random.Random(48), 48, ('v',))),
+         '-b', 'tag,'],
+        ['-f', json.dumps(random_predicate(random.Random(48), 49, ('v',))),
+         '-b', 'tag,'],
+        'filter too large'),
+    # the pool holds the string constants and the candidate key names ("s"
+    # and "tag" here)
+    'pool_2048': (
+        ['-f', _or_eq([('s', 'x' * (2048 - 4))]), '-b', 'tag,'],
+        ['-f', _or_eq([('s', 'x' * (2048 - 3))]), '-b', 'tag,'],
+        'plan constant pool exhausted'),
+    'fields_24': (
+        ['-f', _or_eq([(f, 1) for f in ['v'] + ['f%02d' % i
+                                                for i in range(22)]]),
+         '-b', 'tag,'],
+        ['-f', _or_eq([(f, 1) for f in ['v'] + ['f%02d' % i
+                                                for i in range(23)]]),
+         '-b', 'tag,'],
+        'too many distinct fields'),
+    'components_30': (
+        ['-f', _or_eq([(f, 1) for f in ['v'] + _COMPONENTS_30]),
+         '-b', 'tag,'],
+        ['-f', _or_eq([(f, 1) for f in ['v'] + _COMPONENTS_30 +
+                       ['a.b.c.d.y']]), '-b', 'tag,'],
+        'too many distinct fields in one scan'),
+    'levels_8': (
+        ['-f', _or_eq([('v', 1), ('a.b.c.d.e.f.g.h', 1)]), '-b', 'tag,'],
+        ['-f', _or_eq([('v', 1), ('a.b.c.d.e.f.g.h.i', 1)]), '-b', 'tag,'],
+        'field "a.b.c.d.e.f.g.h.i" has too many dot-separated components'),
+    'breakdowns_12': (
+        ['-b', 'tag,n,s,b,v,opt,a.b,t,c1,c2,c3,c4,'],
+        ['-b', 'tag,n,s,b,v,opt,a.b,t,c1,c2,c3,c4,c5,'],
+        'too many breakdowns'),
+}
+
+# constants of 1-8 bytes beside values of `s` of the same length that share
+# all but their last byte with them (G GF GET GETS GETSA GETSAB GETSABC
+# GETSABCD), then long ones: 48 + 7 * 56 + 44 = 484 bytes padded to words
+_F_SHORT = ['G', 'GE', 'GET', 'GETT', 'GETSA', 'GETSAC', 'GETSABC',
+            'GETSABCE']
+_F_LONG = ['%02d' % i + 'L' * 54 for i in range(7)]
+
+# the F plan's limits (fast.cpp fplan_build), each as (argv at the limit,
+# argv one past it)
+F_LIMITS = {
+    'leaves_16': (
+        ['-f', json.dumps(random_predicate(random.Random(16), 16, ('v',))),
+         '-b', 'tag,'],
+        ['-f', json.dumps(random_predicate(random.Random(16), 17, ('v',))),
+         '-b', 'tag,']),
+    'pool_484': (
+        ['-f', _or_eq([('s', c) for c in _F_SHORT + _F_LONG + ['y' * 44]]),
+         '-b', 'tag,'],
+        ['-f', _or_eq([('s', c) for c in _F_SHORT + _F_LONG + ['y' * 45]]),
+         '-b', 'tag,']),
+    'paths_8': (
+        ['-f', _or_eq([(f, 26) for f in ('v', 'n', 's', 'b', 'opt', 'a.b',
+                                         'nope')]), '-b', 'tag,'],
+        ['-f', _or_eq([(f, 26) for f in ('v', 'n', 's', 'b', 'opt', 'a.b',
+                                         'nope', 't')]), '-b', 'tag,']),
+    'columns_6': (['-b', 'tag,n,s,b,opt,a.b'],
+                  ['-b', 'tag,n,s,b,opt,a.b,v,']),
+    'synthetic_2': (
+        ['-b', 'd1[date,field=t,aggr=lquantize,step=3600],'
+         'd2[date,field=t,aggr=lquantize,step=60]'],
+        ['-b', 'd1[date,field=t,aggr=lquantize,step=3600],'
+         'd2[date,field=t,aggr=lquantize,step=60],'
+         'd3[date,field=t,aggr=lquantize,step=1]']),
+}
+
+# plans the key automaton (plan.cpp FastBuilder) cannot take
+_LONG_KEYS = ['k' + chr(ord('a') + i) + 'z' * 26 for i in range(10)]
+AUTOMATON_LIMITS = {
+    # ten 28-byte keys: more than FAST_MAXSTATES (200) trie states
+    'states': ['-f', _or_eq([('v', 26)] + [(k, 1) for k in _LONG_KEYS]),
+               '-b', 'tag,'],
+    # 13 field contexts (the root, a .. a.b.c.d.e.f.g, x .. x.y.z.w.q), more
+    # than FAST_MAXCTX (12)
+    'contexts': ['-f', _or_eq([('v', 26), ('a.b.c.d.e.f.g.h', 1),
+                               ('x.y.z.w.q.r', 1)]), '-b', 'tag,'],
+    # (no case for FAST_MAXKEYS (48): each path component adds one key name
+    # and each context at most one more, so a plan of at most 30 components
+    # and 12 contexts has at most 41 keys, and the key limit is never the
+    # one a plan exceeds; DESIGN §4)
+}
