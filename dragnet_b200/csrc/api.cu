@@ -675,8 +675,10 @@ int feed_piece(dng_scan *s, const u8 *buf, size_t len, size_t upto, bool pinned)
 		s->carry_len = 0;
 	}
 	if (len > upto) {
+		/* a line is refused once 16 MiB of it, before its newline, have
+		 * to be carried (DESIGN.md section 4) */
 		size_t tail = len - upto;
-		if (s->carry_len + tail > DNG_MAXREC)
+		if (s->carry_len + tail >= DNG_MAXREC)
 			return s->fail(DNG_ELIMIT, "input line longer than 16 MiB");
 		CK(s, cudaMemcpyAsync(s->d_carry + s->carry_len, dst + upto, tail,
 		    cudaMemcpyDeviceToDevice, s->stream));
@@ -1261,7 +1263,7 @@ int dng_scan_feed_device(dng_scan *s, const void *devbuf, size_t len)
 	}
 	if (got[0] == ~0ull) {
 		/* no newline at all: the whole chunk extends the carry */
-		if (s->carry_len + len > DNG_MAXREC)
+		if (s->carry_len + len >= DNG_MAXREC)
 			return s->fail(DNG_ELIMIT, "input line longer than 16 MiB");
 		CK(s, cudaMemcpyAsync(s->d_carry + s->carry_len, d, len,
 		    cudaMemcpyDeviceToDevice, s->stream));
@@ -1271,7 +1273,8 @@ int dng_scan_feed_device(dng_scan *s, const void *devbuf, size_t len)
 	unsigned long long first = got[0], last = got[1];
 	unsigned long long start = 0;
 	if (s->carry_len) {
-		/* finish the carried line in a side buffer */
+		/* finish the carried line in a side buffer (`head` counts its
+		 * newline) */
 		size_t head = (size_t)first + 1;
 		if (s->carry_len + head > DNG_MAXREC)
 			return s->fail(DNG_ELIMIT, "input line longer than 16 MiB");
@@ -1290,7 +1293,7 @@ int dng_scan_feed_device(dng_scan *s, const void *devbuf, size_t len)
 		return s->err_code;
 	if (last < len) {
 		size_t tail = len - (size_t)last;
-		if (tail > DNG_MAXREC)
+		if (tail >= DNG_MAXREC)
 			return s->fail(DNG_ELIMIT, "input line longer than 16 MiB");
 		CK(s, cudaMemcpyAsync(s->d_carry, d + last, tail,
 		    cudaMemcpyDeviceToDevice, s->stream));
