@@ -186,6 +186,11 @@ struct dng_scan {
 	unsigned long long *h_live = nullptr;
 	u8 *d_tmpl = nullptr;
 	u32 tmpl_bytes = 0, ntemplates = 0;
+	/* what learns since d_tmpl was last built resolved, oldest first: the
+	 * first general launch builds d_tmpl from it (an F scan never does) */
+	std::vector<std::pair<std::vector<TCandidate>, std::vector<TResolved>>>
+	    tmpl_pending;
+	u8 *h_blobs = nullptr;		/* pinned staging of the blob uploads */
 	/* the F path (fast.h): its plan, its templates, its miss list */
 	FPlan fplan;
 	FPlan *d_fplan = nullptr;
@@ -253,6 +258,28 @@ __global__ void resolve_pairs_kernel(const DevPlan *plan, const u8 *lines,
 }
 
 /*
+ * A trie blob (tmpl_build, at most TMPL_RESERVE bytes) into a new device buffer
+ * `*dst`, padded to 128 bytes, through half `half` of the pinned staging.  No
+ * wait: the stream orders the copy before every launch that reads the blob.
+ * A half is written again only after the stream has been waited for (the F
+ * half by the next learn, the general half by the build after the next learn),
+ * so the copy out of it has finished by then.
+ */
+int upload_blob(dng_scan *s, int half, std::vector<u8> &blob, u8 **dst)
+{
+	const size_t padded = (blob.size() + 127) & ~(size_t)127;
+	blob.resize(padded, 0);
+	if (!s->h_blobs)
+		CK(s, HOST_ALLOC(&s->h_blobs, 2 * TMPL_RESERVE));
+	u8 *stage = s->h_blobs + half * TMPL_RESERVE;
+	memcpy(stage, blob.data(), padded);
+	CK(s, DEV_ALLOC(s, dst, padded));
+	CK(s, cudaMemcpyAsync(*dst, stage, padded, cudaMemcpyHostToDevice,
+	    s->stream));
+	return 0;
+}
+
+/*
  * The F path's templates (fast.h): the same candidates, their captures indexed
  * by path, compact literals.  `blob` keeps them for the compiled matcher, `t`
  * says what they cover of the sample.
@@ -283,15 +310,54 @@ int learn_ftemplates(dng_scan *s, const std::vector<TCandidate> &cands,
 		if (accepted[i])
 			t.covered += cands[i].count;
 	if (!blob.empty()) {
-		size_t padded = (blob.size() + 127) & ~(size_t)127;
-		blob.resize(padded, 0);
-		CK(s, DEV_ALLOC(s, &s->d_ftmpl, padded));
-		CK(s, cudaMemcpyAsync(s->d_ftmpl, blob.data(), padded,
-		    cudaMemcpyHostToDevice, s->stream));
-		CK(s, cudaStreamSynchronize(s->stream));
-		s->ftmpl_bytes = (u32)padded;
+		/* (the blob this replaces was freed above, after the resolve
+		 * waited for the stream: no launch was reading it) */
+		if (upload_blob(s, 0, blob, &s->d_ftmpl))
+			return s->err_code;
+		s->ftmpl_bytes = (u32)blob.size();
 		s->nftemplates = nt;
 	}
+	return 0;
+}
+
+/*
+ * The general kernels' blob from the learns since it was last built: the
+ * latest learn whose candidates give one, as if every learn had built its own
+ * and one that gives none had left the previous blob in place.
+ */
+void general_blob(const dng_scan *s, std::vector<u8> &blob, u32 *nt)
+{
+	blob.clear();
+	*nt = 0;
+	for (size_t i = s->tmpl_pending.size(); i-- > 0 && blob.empty();)
+		tmpl_build(s->tmpl_pending[i].first, s->tmpl_pending[i].second,
+		    TMPL_RESERVE, blob, nt);
+}
+
+/* d_tmpl for a general launch, if learns since the last build left any */
+int build_general(dng_scan *s)
+{
+	if (s->tmpl_pending.empty())
+		return 0;
+	std::vector<u8> blob;
+	u32 nt = 0;
+	general_blob(s, blob, &nt);
+	s->tmpl_pending.clear();
+	if (blob.empty())
+		return 0;
+	/*
+	 * Only general launches read d_tmpl, and every one since it was last
+	 * built came before the learn that queued this build, which waited for
+	 * the stream: the blob being replaced is not in use, even with F
+	 * launches still running.
+	 */
+	cached_free(s->d_tmpl);
+	s->d_tmpl = nullptr;
+	s->tmpl_bytes = 0;
+	if (upload_blob(s, 1, blob, &s->d_tmpl))
+		return s->err_code;
+	s->tmpl_bytes = (u32)blob.size();
+	s->ntemplates = nt;
 	return 0;
 }
 
@@ -359,32 +425,18 @@ int build_templates(dng_scan *s, const u8 *head, size_t n,
 	if (s->kc.f_ok && learn_ftemplates(s, cands, res, sampled_lines, fblob,
 	    ft))
 		return s->err_code;
-	std::vector<u8> blob;
-	u32 nt = 0;
-	tmpl_build(cands, res, TMPL_RESERVE, blob, &nt);
-	if (blob.empty())
-		return 0;
-	size_t padded = (blob.size() + 127) & ~(size_t)127;
-	blob.resize(padded, 0);
-	/* (the stream is idle here: a blob being replaced is not in use) */
-	cached_free(s->d_tmpl);
-	s->d_tmpl = nullptr;
-	s->tmpl_bytes = 0;
-	CK(s, DEV_ALLOC(s, &s->d_tmpl, padded));
-	CK(s, cudaMemcpyAsync(s->d_tmpl, blob.data(), padded,
-	    cudaMemcpyHostToDevice, s->stream));
-	CK(s, cudaStreamSynchronize(s->stream));
-	s->tmpl_bytes = (u32)padded;
-	s->ntemplates = nt;
+	s->tmpl_pending.emplace_back(std::move(cands), std::move(res));
 	return 0;
 }
 
 /*
  * Sample the head of data[start, nbytes) (device memory): its lines set the
- * kernel geometry, its records the templates.
+ * kernel geometry, its records the templates.  `sample`: that head already
+ * copied to host memory by the caller (with the stream waited for since), or
+ * null.
  */
 int learn_templates(dng_scan *s, const u8 *data, unsigned long long start,
-    unsigned long long nbytes)
+    unsigned long long nbytes, const u8 *sample)
 {
 	s->tmpl_tried = true;
 	if (!kc_wants_sample(s->kc, s->tmpl_enabled))
@@ -393,24 +445,28 @@ int learn_templates(dng_scan *s, const u8 *data, unsigned long long start,
 	    TMPL_SAMPLE_BYTES);
 	/* pinned (and cached) so that the copy is a plain DMA */
 	u8 *hbuf = nullptr;
-	CK(s, HOST_ALLOC(&hbuf, TMPL_SAMPLE_BYTES));
 	struct Release {
 		u8 *p;
 		~Release() { cached_free(p); }
-	} release{hbuf};
-	CK(s, cudaMemcpyAsync(hbuf, data + start, n, cudaMemcpyDeviceToHost,
-	    s->stream));
-	CK(s, cudaStreamSynchronize(s->stream));
+	} release{nullptr};
+	if (!sample) {
+		CK(s, HOST_ALLOC(&hbuf, TMPL_SAMPLE_BYTES));
+		release.p = hbuf;
+		CK(s, cudaMemcpyAsync(hbuf, data + start, n,
+		    cudaMemcpyDeviceToHost, s->stream));
+		CK(s, cudaStreamSynchronize(s->stream));
+		sample = hbuf;
+	}
 	std::vector<u8> fblob;
 	KcTemplates ft;
-	if (s->tmpl_enabled && build_templates(s, hbuf, n, fblob, ft))
+	if (s->tmpl_enabled && build_templates(s, sample, n, fblob, ft))
 		return s->err_code;
-	kc_sample(s->kc, hbuf, n, ft);
+	kc_sample(s->kc, sample, n, ft);
 	if (ft.learned) {
 		s->jit.reset();
 		if (s->jit_mode && !fblob.empty())
-			s->jit = jit_request(jit_source(fblob.data(), fblob.size(),
-			    &s->fplan), (int)s->kc.f_nsl, s->device,
+			s->jit = jit_request(fblob.data(), fblob.size(),
+			    &s->fplan, (int)s->kc.f_nsl, s->device,
 			    (int)s->f_smem_max, s->jit_mode == 2);
 	}
 	return 0;
@@ -567,23 +623,26 @@ int launch_fscan(dng_scan *s, const u8 *data, unsigned long long start,
 	return s->cuda(le, "scan_kernel_f launch");
 }
 
-/* launch the scan kernel over data[start, nbytes) */
+/* launch the scan kernel over data[start, nbytes); `sample`: see
+ * learn_templates */
 int launch_scan(dng_scan *s, const u8 *data, unsigned long long start,
-    unsigned long long nbytes, bool final)
+    unsigned long long nbytes, bool final, const u8 *sample = nullptr)
 {
 	if (nbytes <= start)
 		return 0;
 	if (!s->tmpl_tried) {
-		if (learn_templates(s, data, start, nbytes))
+		if (learn_templates(s, data, start, nbytes, sample))
 			return s->err_code;
 	} else if (s->h_live) {
 		const volatile unsigned long long *lv = s->h_live;
 		const KcLive live = { lv[CTR_LINES], lv[CTR_LONG], lv[CTR_TMPL],
 		    lv[CTR_AGGR], lv[CTR_OVER] };
 		if (kc_counters(s->kc, live, s->tmpl_enabled)) {
-			if (learn_templates(s, data, start, nbytes))
+			if (learn_templates(s, data, start, nbytes, nullptr))
 				return s->err_code;
-			/* the stream is idle: the counters below are current */
+			/* the stream was waited for after the last launch (the
+			 * blob uploads since touch no counter): the counters
+			 * below are current */
 			s->kc.learn_lines = lv[CTR_LINES];
 			s->kc.learn_tmpl = lv[CTR_TMPL];
 		}
@@ -591,6 +650,8 @@ int launch_scan(dng_scan *s, const u8 *data, unsigned long long start,
 	const int kind = kc_pick(s->kc);
 	if (kind == KK_F)
 		return launch_fscan(s, data, start, nbytes, final);
+	if (build_general(s))
+		return s->err_code;
 	ScanArgs a;
 	a.data = data;
 	a.start = start;
@@ -1230,6 +1291,23 @@ int dng_scan_feed_device(dng_scan *s, const void *devbuf, size_t len)
 	cudaSetDevice(s->device);
 	const u8 *d = (const u8 *)devbuf;
 	s->bytes_fed += len;
+	/*
+	 * The first scan of this data starts at its first byte when nothing is
+	 * carried: the head the scan learns its templates from is copied out
+	 * along with the newline search, and arrives with it, in one wait.
+	 */
+	u8 *sample = nullptr;
+	struct Release {
+		u8 *p;
+		~Release() { cached_free(p); }
+	} release{nullptr};
+	if (!s->tmpl_tried && !s->carry_len &&
+	    kc_wants_sample(s->kc, s->tmpl_enabled)) {
+		CK(s, HOST_ALLOC(&sample, TMPL_SAMPLE_BYTES));
+		release.p = sample;
+		CK(s, cudaMemcpyAsync(sample, d, std::min<size_t>(len,
+		    TMPL_SAMPLE_BYTES), cudaMemcpyDeviceToHost, s->stream));
+	}
 	/* locate the first and last newline (windows first, then all) */
 	unsigned long long init[2] = { ~0ull, 0 }, got[2];
 	const unsigned long long W = 1 << 20;
@@ -1289,7 +1367,7 @@ int dng_scan_feed_device(dng_scan *s, const void *devbuf, size_t len)
 		s->carry_len = 0;
 		start = head;
 	}
-	if (launch_scan(s, d, start, last, false))
+	if (launch_scan(s, d, start, last, false, start == 0 ? sample : nullptr))
 		return s->err_code;
 	if (last < len) {
 		size_t tail = len - (size_t)last;
@@ -1515,8 +1593,13 @@ int dng_scan_template_stats(dng_scan *s, uint64_t *templates,
 	unsigned long long c = 0;
 	CK(s, cudaMemcpy(&c, s->d_counters + CTR_TMPL, sizeof (c),
 	    cudaMemcpyDeviceToHost));
-	if (templates)
-		*templates = s->ntemplates;
+	if (templates) {
+		/* (what the general kernels' blob holds once it is built) */
+		std::vector<u8> blob;
+		u32 nt = 0;
+		general_blob(s, blob, &nt);
+		*templates = blob.empty() ? s->ntemplates : nt;
+	}
 	if (templated_records)
 		*templated_records = c;
 	return DNG_OK;
@@ -1641,6 +1724,7 @@ void dng_scan_destroy(dng_scan *s)
 			cudaEventDestroy(s->file_done[i]);
 	}
 	cached_free(s->h_live);
+	cached_free(s->h_blobs);
 	cached_free(s->d_plan);
 	cached_free(s->d_tmpl);
 	cached_free(s->d_fplan);

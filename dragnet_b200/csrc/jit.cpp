@@ -244,11 +244,8 @@ static void plan_source(const FPlan &F, std::string &s)
 	s += " }\n};\n";
 }
 
-std::string jit_source(const u8 *blob, size_t bytes, const FPlan *plan,
-    const char *prelude)
+bool jit_shared(const FPlan *plan)
 {
-	std::string s;
-	s += "/* generated by libdragnet_gpu (jit.cpp) */\n";
 	/*
 	 * One copy of each scanner, called, instead of one inlined into every
 	 * block?  With one or two columns the kernel's loop is a little larger
@@ -260,6 +257,27 @@ std::string jit_source(const u8 *blob, size_t bytes, const FPlan *plan,
 	bool shared = plan && plan->ncols >= 3;
 	if (const char *sh = getenv("DNG_JIT_SHARED"))
 		shared = atoi(sh) == 1;
+	return shared;
+}
+
+std::string jit_key(const u8 *blob, size_t bytes, const FPlan *plan, int nsl,
+    int dev, int smem_max)
+{
+	const int head[5] = { dev, smem_max, nsl, jit_shared(plan) ? 1 : 0,
+	    plan ? 1 : 0 };
+	std::string k((const char *)head, sizeof (head));
+	if (plan)
+		k.append((const char *)plan, sizeof (FPlan));
+	k.append((const char *)blob, bytes);
+	return k;
+}
+
+std::string jit_source(const u8 *blob, size_t bytes, const FPlan *plan,
+    const char *prelude)
+{
+	std::string s;
+	s += "/* generated by libdragnet_gpu (jit.cpp) */\n";
+	const bool shared = jit_shared(plan);
 	if (!prelude && shared)
 		s += "#define DNG_JIT_SHARED_SCAN\n";
 	s += prelude ? prelude : PRELUDE;

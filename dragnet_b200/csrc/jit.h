@@ -14,9 +14,10 @@
  * matcher accepts exactly what fmatch() accepts (same trie, same scanners) and
  * everything it rejects is parsed by the general code.
  *
- * Kernels are cached per process by a hash of the generated source.  Both
- * libraries are dlopen()ed; without them (or with DNG_JIT=0) scans use the
- * interpreted matcher.
+ * Kernels are cached per process by what the generated source and its build
+ * are made from (jit_key), so a scan whose kernel is cached generates no
+ * source.  Both libraries are dlopen()ed; without them (or with DNG_JIT=0)
+ * scans use the interpreted matcher.
  */
 #ifndef DNG_JIT_H
 #define DNG_JIT_H
@@ -43,19 +44,31 @@ struct JitKernels {
 /* the CUDA source of dng_jmatch() for an F trie blob (tmpl_build, compact)
  * and of the plan constant the kernel is specialised to (null: left out);
  * `prelude` replaces the device definitions the generated code builds on
- * (tests/hostcheck compiles the same code for the host with its own) */
+ * (tests/hostcheck compiles the same code for the host with its own).
+ * A pure function of the blob's bytes, the plan's bytes, jit_shared(plan) and
+ * the prelude: the rest it writes out is constant text of this library. */
 std::string jit_source(const u8 *blob, size_t bytes, const FPlan *plan,
     const char *prelude = nullptr);
 
+/* whether the generated matcher calls one shared copy of each wildcard
+ * scanner instead of inlining them (DNG_JIT_SHARED=0|1 forces) */
+bool jit_shared(const FPlan *plan);
+
+/* the cache key of the kernels for an F blob and plan at lane slices of nsl x
+ * 16 bytes on device `dev`: every input of jit_source() and of the build, byte
+ * for byte (no hash, so that different inputs never share a kernel) */
+std::string jit_key(const u8 *blob, size_t bytes, const FPlan *plan, int nsl,
+    int dev, int smem_max);
+
 /*
- * The kernels for this source on device `dev`, from the cache or built now:
- * on the caller's thread if `wait` (then state is 1 or 2 on return), else on a
- * worker thread (state 0 until it is done: the caller keeps using the
- * interpreted matcher meanwhile).  smem_max = dynamic shared memory the
- * kernels may be launched with.
+ * The kernels for this blob and plan on device `dev`, from the cache, or built
+ * now from jit_source(blob, bytes, plan): on the caller's thread if `wait`
+ * (then state is 1 or 2 on return), else on a worker thread (state 0 until it
+ * is done: the caller keeps using the interpreted matcher meanwhile).
+ * smem_max = dynamic shared memory the kernels may be launched with.
  */
-std::shared_ptr<JitKernels> jit_request(const std::string &source, int nsl,
-    int dev, int smem_max, bool wait);
+std::shared_ptr<JitKernels> jit_request(const u8 *blob, size_t bytes,
+    const FPlan *plan, int nsl, int dev, int smem_max, bool wait);
 
 /* load the two compiler libraries now, on this thread (they are dlopen()ed
  * once per process), and compile and link an empty kernel with them once, so

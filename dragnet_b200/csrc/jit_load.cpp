@@ -19,7 +19,7 @@ namespace {
 
 std::mutex g_mu;
 std::condition_variable g_cv;
-std::map<std::pair<int, u64>, std::shared_ptr<JitKernels>> g_cache;
+std::map<std::string, std::shared_ptr<JitKernels>> g_cache;	/* by jit_key */
 
 /*
  * Compiler threads must be joined before the compiler libraries tear
@@ -57,10 +57,8 @@ void join_workers_at_exit()
 	g_workers.join_all();
 }
 
-typedef std::pair<int, u64> CacheKey;
-
 void build_into(std::shared_ptr<JitKernels> k, std::string source, int nsl,
-    int dev, int smem_max, CacheKey key)
+    int dev, int smem_max, std::string key)
 {
 	/* one build at a time; by the time it is this one's turn the scan that
 	 * asked may be gone (short scans, test suites), or the process on its
@@ -114,17 +112,12 @@ void jit_finish()
 	join_workers_at_exit();
 }
 
-std::shared_ptr<JitKernels> jit_request(const std::string &source, int nsl,
-    int dev, int smem_max, bool wait)
+std::shared_ptr<JitKernels> jit_request(const u8 *blob, size_t bytes,
+    const FPlan *plan, int nsl, int dev, int smem_max, bool wait)
 {
-	u64 hsh = 1469598103934665603ull;
-	for (unsigned char c : source)
-		hsh = (hsh ^ c) * 1099511628211ull;
-	hsh ^= (u64)source.size() << 40;
-	hsh = (hsh ^ (u64)nsl) * 1099511628211ull;
+	std::string key = jit_key(blob, bytes, plan, nsl, dev, smem_max);
 	std::unique_lock<std::mutex> g(g_mu);
 	std::shared_ptr<JitKernels> k;
-	const CacheKey key = std::make_pair(dev, hsh);
 	auto it = g_cache.find(key);
 	if (it != g_cache.end()) {
 		k = it->second;
@@ -132,14 +125,14 @@ std::shared_ptr<JitKernels> jit_request(const std::string &source, int nsl,
 		/* (failures are cached too: not tried again for every scan) */
 		k = std::make_shared<JitKernels>();
 		g_cache[key] = k;
+		g.unlock();
+		const std::string source = jit_source(blob, bytes, plan);
 		if (wait) {
-			g.unlock();
 			build_into(k, source, nsl, dev, smem_max, key);
 			g.lock();
 		} else {
 			/* (the libraries loaded and run once, here, and then
 			 * the handler that waits for the thread: see Workers) */
-			g.unlock();
 			jit_prepare();
 			static std::once_flag once;
 			std::call_once(once, [] { atexit(join_workers_at_exit); });

@@ -121,17 +121,16 @@ struct KcTemplates {
 inline void kc_sample(KernelChoice &c, const uint8_t *p, size_t n,
     const KcTemplates &t)
 {
-	size_t longest = 0, run = 0, nl = 0;
-	for (size_t i = 0; i < n; i++) {
-		if (p[i] == '\n') {
-			longest = longest > run ? longest : run;
-			run = 0;
-			nl++;
-		} else {
-			run++;
-		}
+	size_t longest = 0, nl = 0, pos = 0;
+	while (pos < n) {
+		const void *q = memchr(p + pos, '\n', n - pos);
+		const size_t end = q ? (size_t)((const uint8_t *)q - p) : n;
+		longest = longest > end - pos ? longest : end - pos;
+		if (!q)
+			break;
+		nl++;
+		pos = end + 1;
 	}
-	longest = longest > run ? longest : run;
 	const bool short_lines = longest <= DNG_W_MAXLINE;
 	c.mean_line = nl ? (double)n / (double)nl : 224.0;
 	c.wslice = kc_lane_slice(c.mean_line, HUGE_VAL);

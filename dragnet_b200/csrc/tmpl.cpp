@@ -8,7 +8,6 @@
 #include <string.h>
 
 #include <algorithm>
-#include <map>
 
 #include "tmpl.h"
 
@@ -98,16 +97,82 @@ struct SegSink {
 		out.push_back(cur);
 	}
 };
-struct HashSink {		/* FNV-1a over literals and wildcard kinds */
-	u64 h = 1469598103934665603ull;
-	void lit(const u8 *p, u32 n) {
-		for (u32 i = 0; i < n; i++)
-			h = (h ^ p[i]) * 1099511628211ull;
-	}
-	void wild(u8 kind, u32, u32) {
-		h = (h ^ (0x100u + kind)) * 1099511628211ull;
+/* bytes that end a bare scalar in skeleton_walk */
+struct BareEnd {
+	bool t[256];
+	BareEnd() {
+		for (int c = 0; c < 256; c++)
+			t[c] = c == ',' || c == ']' || c == '}' || c == ':' ||
+			    c == '"' || is_ws((u8)c);
 	}
 };
+const BareEnd bare_end;
+
+/*
+ * Does line s[0, n) have the skeleton `segs`?  The walk's state (open
+ * containers, key expected) at any byte depends only on the bytes before it
+ * outside wildcards, so a line whose literal runs are those of `segs`, whose
+ * wildcards start where the walk would start one and end where the walk would
+ * end it, is walked exactly as the line the segments came from: same literal
+ * runs, same wildcard kinds, and it is a JSON text exactly when that one was.
+ *
+ * Starts at segment `k`, whose literal begins at at[k]; records where each
+ * later one begins in at[].  Returns segs.size() if the line matches, else the
+ * segment that does not (the ones before it do).
+ */
+size_t skeleton_match(const u8 *s, size_t n, const std::vector<TSeg> &segs,
+    size_t k, size_t *at)
+{
+	size_t i = at[k];
+	for (; k < segs.size(); k++) {
+		const TSeg &g = segs[k];
+		at[k] = i;
+		const size_t L = g.lit.size();
+		if (n - i < L || memcmp(s + i, g.lit.data(), L) != 0)
+			return k;
+		i += L;
+		if (g.kind == TK_STR) {
+			/* after the opening quote (the literal's last byte): the
+			 * closing one, escapes skipped as the walk does */
+			for (;;) {
+				const u8 *q = (const u8 *)memchr(s + i, '"',
+				    n - i);
+				if (!q)
+					return k;
+				const u8 *b = (const u8 *)memchr(s + i, '\\',
+				    (size_t)(q - (s + i)));
+				if (!b) {
+					i = (size_t)(q - s);
+					break;
+				}
+				i = (size_t)(b - s) + 2;
+				if (i >= n)
+					return k;
+			}
+		} else if (g.kind == TK_BARE) {
+			/* the walk takes a bare scalar from any other byte */
+			if (i >= n || bare_end.t[s[i]] || s[i] == '{' ||
+			    s[i] == '[')
+				return k;
+			while (i < n && !bare_end.t[s[i]])
+				i++;
+		} else {
+			return i == n ? segs.size() : k;
+		}
+	}
+	return k;
+}
+
+/* how many leading segments two skeletons have in common */
+size_t common_segs(const std::vector<TSeg> &a, const std::vector<TSeg> &b)
+{
+	size_t k = 0;
+	while (k < a.size() && k < b.size() && a[k].kind == b[k].kind &&
+	    a[k].lit == b[k].lit)
+		k++;
+	return k;
+}
+
 }
 
 bool tmpl_skeletonize(const u8 *s, u32 n, std::vector<TSeg> &out)
@@ -123,10 +188,17 @@ void tmpl_candidates(const u8 *data, size_t len, size_t maxk,
 	out.clear();
 	if (nlines_out)
 		*nlines_out = 0;
-	/* count shapes by a hash of their skeleton; only the first line of each
-	 * distinct shape is broken into segments */
-	std::map<u64, size_t> seen;
-	size_t pos = 0, nlines = 0;
+	/*
+	 * Count lines by skeleton: a line is tried against the shapes already
+	 * seen (the last one matched first), and only a line that has none of
+	 * them is walked.  Where a shape fails at segment k, the next one goes
+	 * on from the segments it shares with that one (up to k), and is passed
+	 * over if it shares segment k as well.
+	 */
+	size_t pos = 0, nlines = 0, last = 0;
+	std::vector<TSeg> segs;
+	std::vector<std::vector<size_t>> common;	/* common_segs per pair */
+	std::vector<size_t> at(TMPL_MAX_LINE + 2);
 	while (pos < len && nlines < 8192) {
 		const u8 *nl = (const u8 *)memchr(data + pos, '\n', len - pos);
 		if (!nl)
@@ -137,21 +209,47 @@ void tmpl_candidates(const u8 *data, size_t len, size_t maxk,
 		nlines++;
 		if (n == 0 || n > TMPL_MAX_LINE)
 			continue;
-		HashSink hs;
-		if (!skeleton_walk(line, (u32)n, hs))
-			continue;
-		auto it = seen.find(hs.h);
-		if (it != seen.end()) {
-			out[it->second].count++;
+		size_t hit = out.size();
+		if (!out.empty()) {
+			/* the shape tried last, where it failed (at[] holds
+			 * where its segments up to that one begin) */
+			size_t prev = last;
+			at[0] = 0;
+			size_t fail = skeleton_match(line, n, out[last].segs, 0,
+			    at.data());
+			if (fail == out[last].segs.size())
+				hit = last;
+			for (size_t k = 0; hit == out.size() && k < out.size();
+			    k++) {
+				const size_t c = common[prev][k];
+				if (k == last || c > fail)
+					continue;
+				fail = skeleton_match(line, n, out[k].segs, c,
+				    at.data());
+				prev = k;
+				if (fail == out[k].segs.size())
+					hit = k;
+			}
+		}
+		if (hit < out.size()) {
+			out[hit].count++;
+			last = hit;
 			continue;
 		}
-		if (seen.size() >= 256)
+		if (out.size() >= 256 || !tmpl_skeletonize(line, (u32)n, segs))
 			continue;
-		seen[hs.h] = out.size();
 		TCandidate c;
 		c.sample.assign((const char *)line, n);
-		tmpl_skeletonize(line, (u32)n, c.segs);
+		c.segs = segs;
 		c.count = 1;
+		last = out.size();
+		common.emplace_back();
+		for (size_t k = 0; k < out.size(); k++) {
+			const size_t m = common_segs(out[k].segs, segs);
+			common[k].push_back(m);
+			common.back().push_back(m);
+		}
+		common.back().push_back(segs.size());
 		out.push_back(c);
 	}
 	std::stable_sort(out.begin(), out.end(),
