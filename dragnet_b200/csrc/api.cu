@@ -482,22 +482,17 @@ u32 tier2_slots(size_t room)
 	return n;
 }
 
-/* the F kernel for lane slices of nsl x 16 bytes, and its per-warp shared
- * memory */
-const void *fkernel(u32 nsl, u32 *warp_bytes)
+/* the F kernel for lane slices of nsl x 16 bytes */
+const void *fkernel(u32 nsl)
 {
 	switch (nsl) {
 	case 7:
-		*warp_bytes = FWarpSmem<7>::BYTES;
 		return (const void *)scan_kernel_f<7>;
 	case 9:
-		*warp_bytes = FWarpSmem<9>::BYTES;
 		return (const void *)scan_kernel_f<9>;
 	case 11:
-		*warp_bytes = FWarpSmem<11>::BYTES;
 		return (const void *)scan_kernel_f<11>;
 	default:
-		*warp_bytes = FWarpSmem<13>::BYTES;
 		return (const void *)scan_kernel_f<13>;
 	}
 }
@@ -574,8 +569,9 @@ int launch_fscan(dng_scan *s, const u8 *data, unsigned long long start,
 	cudaEventRecord(e0, s->stream);
 	/* the matcher compiled for these templates, once it is there */
 	const bool jit = s->jit && s->jit->state.load() == 1 && s->ftmpl_bytes;
-	u32 warp_bytes = 0;
-	const void *kern = fkernel(nsl, &warp_bytes);
+	a.wunits = fwindow_units(nsl, nw);
+	const u32 warp_bytes = fwarp_bytes(a.wunits);
+	const void *kern = fkernel(nsl);
 	/* (the compiled matcher has the templates in its code: no trie in shared
 	 * memory, more of it for the tally cache) */
 	const u32 tmpl_room = jit ? 0 : (u32)TMPL_RESERVE;
@@ -885,8 +881,8 @@ int dng_scan_open(const dng_plan *plan, int device, dng_scan **out, char *err,
 		s->f_smem_max = (u32)prop.sharedMemPerBlockOptin - 1024;
 		cudaError_t fe = cudaFuncSetAttribute(scan_miss_kernel,
 		    cudaFuncAttributeMaxDynamicSharedMemorySize, (int)s->f_smem_max);
-		for (u32 nsl = 7, wb; nsl <= 13 && fe == cudaSuccess; nsl += 2)
-			fe = cudaFuncSetAttribute(fkernel(nsl, &wb),
+		for (u32 nsl = 7; nsl <= 13 && fe == cudaSuccess; nsl += 2)
+			fe = cudaFuncSetAttribute(fkernel(nsl),
 			    cudaFuncAttributeMaxDynamicSharedMemorySize,
 			    (int)s->f_smem_max);
 		if ((rc = s->cuda(fe, "cudaFuncSetAttribute")))
@@ -914,8 +910,7 @@ int dng_scan_open(const dng_plan *plan, int device, dng_scan **out, char *err,
 		}
 		/* (a plan with many capture rows leaves the F kernel's buffers
 		 * no room) */
-		u32 warp_bytes = 0;
-		fkernel(13, &warp_bytes);
+		const u32 warp_bytes = fwarp_bytes(fwindow_units(13, DNG_F_NW));
 		const bool f_fits = fkernel_smem(warp_bytes, TMPL_RESERVE, 32,
 		    DNG_SSLOTS_MIN, s->fplan.nrows, DNG_F_NW) <= s->f_smem_max;
 		const bool warp_fits = SMEM_W_FIXED + s->plan_bytes + TMPL_RESERVE +

@@ -6,18 +6,20 @@
  * Geometry: one persistent 896-thread CTA per SM; every WARP is its own
  * pipeline, as in scan_kernel_w, over SEGMENTS of consecutive chunks:
  *
- *   - a chunk is 32 lane slices of NSL x 16 bytes (the host picks NSL so that
- *     a chunk holds just under 32 average records), staged by one TMA bulk
- *     copy into the warp's private buffer behind a 512-byte pre-lap;
- *   - the record that straddles two chunks of a segment never goes back to
- *     HBM: before the next chunk is staged, the warp copies the last 512 bytes
- *     of its buffer into the pre-lap (shared -> shared) and carries the start
- *     of the open record over.  Only a segment's first chunk stages its
- *     pre-lap from HBM;
+ *   - a chunk is 32 x NSL x 16 bytes (the host picks NSL so that a chunk
+ *     holds just under 32 average records); a segment owns the records whose
+ *     newline lies in its chunks;
+ *   - the warp walks its segment in WINDOWS of 32 lane slices of `wunits` x
+ *     16 bytes, each staged by one TMA bulk copy into its private buffer.  The
+ *     first stages the 512-byte pre-lap before the segment with it, to find
+ *     where the open record starts; every later one starts at the first
+ *     record not yet taken (16-byte aligned), so it holds 32 complete records
+ *     where the lines allow and every lane of the record pass has one.  The
+ *     bytes after the 32nd come again with the next window, from L2;
  *   - newline index: every lane tests its slice 16 bytes at a time with one
  *     "any byte == '\n'" SWAR test per word (exact analysis only where it
- *     fires), a shuffle scan orders the hits, lanes write their (<= 4)
- *     positions; record r of the chunk goes to lane r;
+ *     fires), a shuffle scan orders the hits, lanes write their positions;
+ *     record r of the window goes to lane r;
  *   - fmatch() -> fstage() -> fkey_hash() / tally (fast.cuh): captures are one
  *     word per path in shared memory ([path][thread]: conflict free), the key
  *     is hashed and compared in place against the CTA's tally cache;
@@ -25,7 +27,8 @@
  *     (absolute offsets) and parsed by scan_miss_kernel right after this
  *     kernel; if the list is full it is parsed here, out of line, from HBM.
  *
- * Bound: HBM read of the input, once (+ 512 bytes per segment).
+ * Bound: HBM read of the input, once (+ 512 bytes per segment); the windows
+ * read it from L2 once more per 32 records, in part.
  */
 #ifndef DNG_FAST_KERNEL_CUH
 #define DNG_FAST_KERNEL_CUH
@@ -60,6 +63,8 @@ struct FScanArgs {
 	unsigned long long *counters;
 	GTable tab;
 	u32 nchunks, seg;		/* chunks, chunks per segment */
+	u32 wunits;			/* window: lane slices of NSL + 1 or
+					 * NSL + 2 16-byte units (fwindow_units) */
 	u32 final;
 	u32 s1slots, sslots;
 	u32 nrows;			/* capture rows (FPlan::nrows) */
@@ -69,17 +74,31 @@ struct FScanArgs {
 	u32 *seg_next;			/* segment queue: zero at launch */
 };
 
-/* per-warp shared memory: buffer, newline positions, mbarrier */
-template <int NSL>
-struct FWarpSmem {
-	static constexpr u32 CHUNK = 32 * 16 * NSL;
-	static constexpr u32 BUF = DNG_F_PRE + CHUNK + DNG_F_SLACK;
-	static constexpr u32 BYTES = (BUF + 2 * DNG_F_NLCAP + 16 + 127) & ~127u;
-};
+/*
+ * The window's lane slices, in 16-byte units, for chunks of nsl-unit slices
+ * and nw warps per CTA.  A chunk holds just under 32 average records, and so
+ * does pre-lap + chunk (nsl + 1 units) once a window starts up to 15 bytes
+ * before its first record: too often for a segment to take fewer passes than
+ * it has chunks (tools/f_passes.py).  512 bytes more (nsl + 2, odd like nsl:
+ * the lanes' 16-byte loads are free of bank conflicts) hold 32; fewer warps
+ * than DNG_F_NW leave the room for them, DNG_F_NW do not.
+ */
+static inline u32 fwindow_units(u32 nsl, u32 nw)
+{
+	return nw < DNG_F_NW ? nsl + 2 : nsl + 1;
+}
+
+/* per-warp shared memory: window, the quotes behind it, newline positions,
+ * mbarrier */
+__host__ __device__ __forceinline__ u32 fwarp_bytes(u32 wunits)
+{
+	return (32 * 16 * wunits + DNG_F_SLACK + 2 * DNG_F_NLCAP + 16 + 127) &
+	    ~127u;
+}
 
 static constexpr u32 FPLAN_SMEM = (sizeof (FPlan) + 127) & ~127u;
 
-/* (warp_bytes = FWarpSmem<NSL>::BYTES; nw = warps of the launch: DNG_F_NW,
+/* (warp_bytes = fwarp_bytes(wunits); nw = warps of the launch: DNG_F_NW,
  * or fewer -- the capture rows keep their stride -- when the tally cache
  * needs the room) */
 static inline size_t fkernel_smem(u32 warp_bytes, u32 tmpl_bytes, u32 s1slots,
@@ -403,8 +422,8 @@ extern "C" __device__ unsigned dng_jmatch(unsigned ra, unsigned len,
 template <int NSL, bool JIT>
 __device__ __forceinline__ void fscan_body(const FScanArgs &a)
 {
-	typedef FWarpSmem<NSL> WS;
-	constexpr u32 CHUNK = WS::CHUNK, SLICE = 16 * NSL, D0 = DNG_F_PRE;
+	constexpr u32 CHUNK = 32 * 16 * NSL, D0 = DNG_F_PRE;
+	const u32 SLICE = 16 * a.wunits, W = 32 * SLICE;
 	extern __shared__ __align__(128) u8 smem[];
 #ifdef DNG_JIT_HOT
 	const FPlan &F = dng_jplan;
@@ -426,11 +445,11 @@ __device__ __forceinline__ void fscan_body(const FScanArgs &a)
 
 	const u32 tid = threadIdx.x;
 	const u32 lane = tid & 31, wid = tid >> 5;
-	/* this warp's buffer, newline positions (u16) and mbarrier: shared
+	/* this warp's window, newline positions (u16) and mbarrier: shared
 	 * addresses */
-	const u32 sb = smem_u32(sp) + wid * WS::BYTES;
-	const u32 nlpos = sb + WS::BUF;
-	const u32 mbar = sb + WS::BUF + 2 * DNG_F_NLCAP;
+	const u32 sb = smem_u32(sp) + wid * fwarp_bytes(a.wunits);
+	const u32 nlpos = sb + W + DNG_F_SLACK;
+	const u32 mbar = nlpos + 2 * DNG_F_NLCAP;
 
 	{	/* plan, templates -> shared; clear the tally cache */
 		const uint4 *src = (const uint4 *)a.fplan;
@@ -452,7 +471,7 @@ __device__ __forceinline__ void fscan_body(const FScanArgs &a)
 		/* the quotes after the buffer that end a runaway string scan
 		 * (fscan.cuh) */
 		if (lane < DNG_F_SLACK / 4)
-			sts32(sb + D0 + CHUNK + 4 * lane, 0x22222222u);
+			sts32(sb + W + 4 * lane, 0x22222222u);
 	}
 	__syncthreads();
 
@@ -484,86 +503,67 @@ __device__ __forceinline__ void fscan_body(const FScanArgs &a)
 	const u32 nseg = (a.nchunks + a.seg - 1) / a.seg;
 
 	for (u32 seg = gw; seg < nseg; ) {
-		const u32 ch0 = seg * a.seg;
-		const u32 ch1 = min(ch0 + a.seg, a.nchunks);
-		/* the open record: where it starts in the buffer (may be
-		 * negative: before it), and in the input if that is known */
-		int beg0 = 0;
-		unsigned long long open_abs = ~0ull;
-		for (u32 ch = ch0; ch < ch1; ch++) {
-			const unsigned long long g0 = (unsigned long long)ch * CHUNK;
-			const u32 dlen = (u32)min((unsigned long long)CHUNK,
-			    a.nbytes - g0);
+		/* the segment's bytes: [g0, g1) */
+		const unsigned long long g0 = (unsigned long long)seg * a.seg *
+		    CHUNK;
+		const unsigned long long g1 = min(g0 + (unsigned long long)a.seg *
+		    CHUNK, a.nbytes);
+		/* the window [base, base + W); `next`: the first byte no pass
+		 * has looked at; the open record's start, if it is known */
+		unsigned long long base = g0 ? g0 - D0 : 0;
+		unsigned long long next = g0 ? g0 : a.start;
+		unsigned long long open_abs = a.start;
+		for (bool first = true;; first = false) {
+			const u32 dlen = (u32)min((unsigned long long)W,
+			    a.nbytes - base);
 			const u32 bulk = dlen & ~15u;
-			const bool first = ch == ch0;
 
 			__syncwarp();
-			if (!first) {
-				/* the tail of the previous chunk becomes the
-				 * pre-lap of this one */
-				const uint4 v = lds128(sb + D0 + CHUNK - DNG_F_PRE +
-				    16 * lane);
-				__syncwarp();
-				sts128(sb + 16 * lane, v);
-				__syncwarp();
-			}
 			if (lane == 0) {
-				const u32 pre = (first && g0) ? DNG_F_PRE : 0;
 				asm volatile("fence.proxy.async.shared::cta;"
 				    ::: "memory");
-				if (bulk + pre) {
-					mbar_expect_tx_sa(mbar, bulk + pre);
-					if (bulk)
-						tma_load_1d_sa(sb + D0, a.data + g0,
-						    bulk, mbar);
-					if (pre)
-						tma_load_1d_sa(sb, a.data + g0 -
-						    DNG_F_PRE, DNG_F_PRE, mbar);
+				if (bulk) {
+					mbar_expect_tx_sa(mbar, bulk);
+					tma_load_1d_sa(sb, a.data + base, bulk,
+					    mbar);
 				}
-				/* start pulling this warp's next chunk into L2 */
-				const unsigned long long nx = g0 + CHUNK;
-				if (ch + 1 < ch1 && nx + CHUNK <= a.nbytes)
-					asm volatile("cp.async.bulk.prefetch.L2."
-					    "global [%0], %1;" :: "l"(a.data + nx),
-					    "r"(CHUNK) : "memory");
 			}
 			for (u32 i = bulk + lane; i < dlen; i += 32)
-				sts8(sb + D0 + i, a.data[g0 + i]);
-			/* (a short last chunk: the sentinel right behind it) */
-			if (dlen < CHUNK && lane < 16)
-				sts8(sb + D0 + dlen + lane, '"');
-			if (bulk || (first && g0)) {
+				sts8(sb + i, a.data[base + i]);
+			/* (a short last window: the sentinel right behind it) */
+			if (dlen < W && lane < 16)
+				sts8(sb + dlen + lane, '"');
+			if (bulk) {
 				mbar_wait_sa(mbar, parity);
 				parity ^= 1;
 			}
 			__syncwarp();
 
-			/* valid bytes of the buffer: [lo, hi) */
-			const u32 lo = g0 ? 0 : D0 + (u32)a.start;
-			const u32 hi = D0 + dlen;
-			if (first) {
+			/* the bytes whose newlines this pass takes: [lo, hi) of
+			 * the window (those after the segment are the next
+			 * one's) */
+			const u32 lo = (u32)(next - base);
+			const u32 hi = (u32)(min(base + dlen, g1) - base);
+			if (first && g0) {
 				/* where the open record starts: after the last
 				 * newline of the pre-lap, which the lanes search
 				 * together (16 bytes each) */
-				beg0 = (int)lo;
-				open_abs = a.start;
-				if (g0) {
-					const uint4 v = lds128(sb + D0 - 16 * (lane + 1));
-					const u32 wd[4] = { v.x, v.y, v.z, v.w };
-					u32 mine = 0;
+				const uint4 v = lds128(sb + D0 - 16 * (lane + 1));
+				const u32 wd[4] = { v.x, v.y, v.z, v.w };
+				u32 mine = 0;
 #pragma unroll
-					for (int j = 3; j >= 0; j--) {
-						const u32 mk = nl_mask(wd[j]);
-						if (mk && !mine)
-							mine = D0 - 16 * (lane + 1) +
-							    4 * j + ((31 - __clz(mk)) >> 3) + 1;
-					}
-					const u32 best = __reduce_max_sync(0xffffffffu,
-					    mine);
-					beg0 = best ? (int)best : -1;
-					open_abs = best ? g0 - D0 + best : ~0ull;
+				for (int j = 3; j >= 0; j--) {
+					const u32 mk = nl_mask(wd[j]);
+					if (mk && !mine)
+						mine = D0 - 16 * (lane + 1) +
+						    4 * j + ((31 - __clz(mk)) >> 3) + 1;
 				}
+				const u32 best = __reduce_max_sync(0xffffffffu, mine);
+				open_abs = best ? base + best : ~0ull;
 			}
+			/* ... and in the window (-1: before it, or unknown) */
+			const int beg0 = open_abs != ~0ull && open_abs >= base ?
+			    (int)(open_abs - base) : -1;
 
 			/* ---- newline index ---- */
 			/*
@@ -573,10 +573,13 @@ __device__ __forceinline__ void fscan_body(const FScanArgs &a)
 			 * -- once a shuffle scan has ordered the lanes -- to write
 			 * the positions.
 			 */
-			const u32 c0 = D0 + lane * SLICE;
+			const u32 c0 = lane * SLICE;
 			u32 hot = 0, cnt = 0, one = 0;
 #pragma unroll
-			for (u32 j = 0; j < (u32)NSL; j++) {
+			for (u32 j = 0; j < (u32)NSL + 2; j++) {
+				/* (slices of NSL + 1 or NSL + 2 units) */
+				if (j == NSL + 1 && a.wunits == NSL + 1)
+					break;
 				/* any byte <= '\n' in these 16?  (b - 0x0b borrows
 				 * exactly for those; a borrow into the next byte can
 				 * only add a flag) */
@@ -592,30 +595,24 @@ __device__ __forceinline__ void fscan_body(const FScanArgs &a)
 			for (u32 hm = hot; hm; hm &= hm - 1) {
 				const u32 p = c0 + 16 * (__ffs(hm) - 1);
 				const uint4 v = lds128(sb + p);
-				if (p >= lo && p + 16 <= hi) {
-					const u32 m0 = nl_mask(v.x), m1 = nl_mask(v.y);
-					const u32 m2 = nl_mask(v.z), m3 = nl_mask(v.w);
-					const u32 k = __popc(m0) + __popc(m1) +
-					    __popc(m2) + __popc(m3);
-					/* (the usual case, one newline per lane: its
-					 * position right away) */
-					if (k == 1)
-						one = p + (m0 ? 0 : m1 ? 4 : m2 ? 8 : 12) +
-						    ((__ffs(m0 | m1 | m2 | m3) - 1) >> 3);
-					cnt += k;
-				} else {
-					/* the ends of the input: byte by byte */
-					for (u32 x = 0; x < 16; x++)
-						cnt += p + x >= lo && p + x < hi &&
-						    lds8(sb + p + x) == '\n';
+				u32 m0 = nl_mask(v.x), m1 = nl_mask(v.y);
+				u32 m2 = nl_mask(v.z), m3 = nl_mask(v.w);
+				if (p < lo || p + 16 > hi) {
+					/* the ends of the pass */
+					m0 &= byte_range_mask(p, lo, hi);
+					m1 &= byte_range_mask(p + 4, lo, hi);
+					m2 &= byte_range_mask(p + 8, lo, hi);
+					m3 &= byte_range_mask(p + 12, lo, hi);
 				}
+				const u32 k = __popc(m0) + __popc(m1) + __popc(m2) +
+				    __popc(m3);
+				/* (the usual case, one newline per lane: its
+				 * position right away) */
+				if (k == 1)
+					one = p + (m0 ? 0 : m1 ? 4 : m2 ? 8 : 12) +
+					    ((__ffs(m0 | m1 | m2 | m3) - 1) >> 3);
+				cnt += k;
 			}
-			/* an unterminated final line ends at a virtual newline:
-			 * it is never templated (nothing terminates its scans) */
-			const bool lastch = ch + 1 == a.nchunks;
-			bool vnl = false;
-			if (lastch && a.final && hi > lo)
-				vnl = lds8(sb + hi - 1) != '\n';
 
 			u32 incl = cnt;
 #pragma unroll
@@ -630,15 +627,15 @@ __device__ __forceinline__ void fscan_body(const FScanArgs &a)
 			if (dense) {
 				/*
 				 * Degenerate input (lines of a few bytes): one lane
-				 * walks the chunk and hands every record to the
+				 * walks the window and hands every record to the
 				 * general parser.
 				 */
 				if (lane == 0) {
 					unsigned long long b = open_abs;
-					for (u32 p = max(lo, D0); p < hi; p++) {
+					for (u32 p = lo; p < hi; p++) {
 						if (lds8(sb + p) != '\n')
 							continue;
-						const unsigned long long e = g0 - D0 + p;
+						const unsigned long long e = base + p;
 						fmiss_put(a, stab, atomicAdd(a.miss_n, 1u),
 						    b, e);
 						b = e + 1;
@@ -646,17 +643,10 @@ __device__ __forceinline__ void fscan_body(const FScanArgs &a)
 					open_abs = b;
 				}
 				open_abs = __shfl_sync(0xffffffffu, open_abs, 0);
-				/* (beg0 of the next chunk is recomputed below) */
-				int last = -1;
-				for (int p = (int)hi - 1; p >= (int)max(lo, D0); p--)
-					if (lds8(sb + p) == '\n') {
-						last = p;
-						break;
-					}
-				if (last >= 0)
-					beg0 = last + 1;
+				next = open_abs;
 			} else if (total) {
-				if (cnt == 1 && one) {
+				/* (cnt == 1: from a unit of one newline) */
+				if (cnt == 1) {
 					sts16(nlpos + 2 * mybase, one);
 				} else if (cnt) {
 					u32 idx = mybase;
@@ -678,100 +668,118 @@ __device__ __forceinline__ void fscan_body(const FScanArgs &a)
 					}
 				}
 				__syncwarp();
+				/* the first 32 records, one per lane */
+				const u32 take = min(total, 32u);
+				if (lane == 0 && total > 32) {
+					/* what the next window adds to this
+					 * one: into L2 while the records are
+					 * matched */
+					const unsigned long long nb = (base +
+					    lds16(nlpos + 2 * 31) + 1) & ~15ull;
+					if (nb + W <= a.nbytes)
+						asm volatile("cp.async.bulk."
+						    "prefetch.L2.global [%0], %1;"
+						    :: "l"(a.data + base + W),
+						    "r"((u32)(nb - base)) : "memory");
+				}
 
-				for (u32 rb = 0; rb < total; rb += 32) {
-					const u32 r = rb + lane;
-					const bool have = r < total;
-					int beg = 0;
-					u32 end = 0;
-					if (have) {
-						end = lds16(nlpos + 2 * r);
-						beg = r ? (int)lds16(nlpos + 2 * r - 2) + 1 :
-						    beg0;
-					}
-					/* (captures carry 12-bit offsets and lengths) */
-					const bool inbuf = have && beg >= 0 &&
-					    end - (u32)beg <= F_MAXLINE;
-					const u32 len = inbuf ? end - (u32)beg : 0;
-					m.ra = sb + (inbuf ? (u32)beg : 0);
-					u32 defmask = 0;
-					u32 fo = FO_MISS;
-					bool matched;
-					if (JIT) {
-						const u32 r_ = dng_jmatch(m.ra, len, inbuf,
-						    m.caps);
-						matched = r_ & 1;
-						defmask = r_ >> 1;
-					} else {
-						matched = use_tmpl &&
-						    fmatch(m, len, inbuf, defmask);
-					}
-					if (matched) {
-						double s0, s1;
-						fo = fstage(m, F, defmask, s0, s1);
-						u32 h = 0, klen = 0, slow = 0;
-						if (fo == FO_AGGR && (!fprep(m, F, defmask,
-						    s0, s1, slow) || !fkey_hash(m, F,
-						    defmask, h, klen)))
-							fo = FO_MISS;
-						if (fo == FO_AGGR) {
-							if (slow)
-								atomicAdd(&s_drop[1], 1u);
-							ftally(m, F, (const FPlan *)smem, defmask,
-							    h, klen, stab, a.tab,
-							    smem_u32(&s_drop[15]));
-						}
-					}
-					const bool done = fo != FO_MISS;
-					ntmpl += __popc(__ballot_sync(0xffffffffu, done));
-					naggr += __popc(__ballot_sync(0xffffffffu,
-					    fo == FO_AGGR));
-					{
-						/* dropped records: one shared atomic per
-						 * outcome present in the warp */
-						u32 dm = __ballot_sync(0xffffffffu,
-						    fo >= FO_DS_FILTERED);
-						while (dm) {
-							const u32 f0 = __shfl_sync(0xffffffffu,
-							    fo, __ffs(dm) - 1);
-							const u32 same = __ballot_sync(
-							    0xffffffffu, fo == f0);
-							if (lane == 0)
-								atomicAdd(&s_drop[f0],
-								    (u32)__popc(same));
-							dm &= ~same;
-						}
-					}
-					/* what the F path did not take */
-					const bool miss = have && !done;
-					const u32 mm = __ballot_sync(0xffffffffu, miss);
-					if (mm) {
-						u32 base = 0;
-						if (lane == 0)
-							base = atomicAdd(a.miss_n,
-							    (u32)__popc(mm));
-						base = __shfl_sync(0xffffffffu, base, 0);
-						if (miss)
-							fmiss_put(a, stab, base +
-							    __popc(mm & ltmask), r ? g0 - D0 +
-							    (u32)beg : open_abs, g0 - D0 + end);
+				const u32 r = lane;
+				const bool have = r < take;
+				int beg = 0;
+				u32 end = 0;
+				if (have) {
+					end = lds16(nlpos + 2 * r);
+					beg = r ? (int)lds16(nlpos + 2 * r - 2) +
+					    1 : beg0;
+				}
+				/* (captures carry 12-bit offsets and lengths) */
+				const bool inbuf = have && beg >= 0 &&
+				    end - (u32)beg <= F_MAXLINE;
+				const u32 len = inbuf ? end - (u32)beg : 0;
+				m.ra = sb + (inbuf ? (u32)beg : 0);
+				u32 defmask = 0;
+				u32 fo = FO_MISS;
+				bool matched;
+				if (JIT) {
+					const u32 r_ = dng_jmatch(m.ra, len, inbuf,
+					    m.caps);
+					matched = r_ & 1;
+					defmask = r_ >> 1;
+				} else {
+					matched = use_tmpl &&
+					    fmatch(m, len, inbuf, defmask);
+				}
+				if (matched) {
+					double s0, s1;
+					fo = fstage(m, F, defmask, s0, s1);
+					u32 h = 0, klen = 0, slow = 0;
+					if (fo == FO_AGGR && (!fprep(m, F, defmask,
+					    s0, s1, slow) || !fkey_hash(m, F,
+					    defmask, h, klen)))
+						fo = FO_MISS;
+					if (fo == FO_AGGR) {
+						if (slow)
+							atomicAdd(&s_drop[1], 1u);
+						ftally(m, F, (const FPlan *)smem, defmask,
+						    h, klen, stab, a.tab,
+						    smem_u32(&s_drop[15]));
 					}
 				}
+				const bool done = fo != FO_MISS;
+				ntmpl += __popc(__ballot_sync(0xffffffffu, done));
+				naggr += __popc(__ballot_sync(0xffffffffu,
+				    fo == FO_AGGR));
+				{
+					/* dropped records: one shared atomic per
+					 * outcome present in the warp */
+					u32 dm = __ballot_sync(0xffffffffu,
+					    fo >= FO_DS_FILTERED);
+					while (dm) {
+						const u32 f0 = __shfl_sync(0xffffffffu,
+						    fo, __ffs(dm) - 1);
+						const u32 same = __ballot_sync(
+						    0xffffffffu, fo == f0);
+						if (lane == 0)
+							atomicAdd(&s_drop[f0],
+							    (u32)__popc(same));
+						dm &= ~same;
+					}
+				}
+				/* what the F path did not take */
+				const bool miss = have && !done;
+				const u32 mm = __ballot_sync(0xffffffffu, miss);
+				if (mm) {
+					u32 mb = 0;
+					if (lane == 0)
+						mb = atomicAdd(a.miss_n,
+						    (u32)__popc(mm));
+					mb = __shfl_sync(0xffffffffu, mb, 0);
+					if (miss)
+						fmiss_put(a, stab, mb +
+						    __popc(mm & ltmask), r ? base +
+						    (u32)beg : open_abs, base + end);
+				}
 				__syncwarp();
-				const u32 lastnl = lds16(nlpos + 2 * (total - 1));
-				beg0 = (int)lastnl + 1;
-				open_abs = g0 - D0 + lastnl + 1;
-				__syncwarp();
+				/* the cursor: past the last record taken */
+				open_abs = next = base +
+				    lds16(nlpos + 2 * (take - 1)) + 1;
+			} else {
+				/* no newline: the open record goes on past the
+				 * window */
+				next = base + dlen;
 			}
-			if (vnl && lane == 0) {
-				/* the unterminated tail [open, end of input) */
-				fmiss_put(a, stab, atomicAdd(a.miss_n, 1u), open_abs,
-				    a.nbytes);
-			}
-			/* the open record, seen from the next chunk's buffer */
-			beg0 -= (int)CHUNK;
-			if (beg0 < 0)
-				beg0 = -1;
+			/* every newline of the segment taken? */
+			if ((dense || total <= 32) && base + dlen >= g1)
+				break;
+			base = next & ~15ull;
+		}
+		/* an unterminated final line ends at a virtual newline: it is
+		 * never templated (nothing terminates its scans) */
+		if (g1 == a.nbytes && a.final && lane == 0 &&
+		    lds8(sb + (u32)(a.nbytes - 1 - base)) != '\n') {
+			/* the tail [open, end of input) */
+			fmiss_put(a, stab, atomicAdd(a.miss_n, 1u), open_abs,
+			    a.nbytes);
 		}
 		/* the next segment nobody has taken yet */
 		if (lane == 0)
