@@ -205,6 +205,12 @@ struct dng_scan {
 	u32 *d_miss_n = nullptr;
 	u32 miss_cap = 0;
 	unsigned long long seen_tmpl = 0;
+	/* a scan over several devices (dng_scan_open_devices) holds no device
+	 * state of its own: it records the files fed, with their sizes, and
+	 * at finish cuts them into one byte range per shard */
+	bool multi = false;
+	std::vector<dng_scan *> shards;
+	std::vector<std::pair<std::string, size_t>> files;
 	std::string err;
 	int err_code = 0;
 
@@ -1003,10 +1009,52 @@ int dng_scan_open(const dng_plan *plan, int device, dng_scan **out, char *err,
 	return DNG_OK;
 }
 
+int dng_scan_open_devices(const dng_plan *plan, const int *devices, int n,
+    dng_scan **out, char *err, size_t errlen)
+{
+	if (!plan || !devices || n <= 0 || !out) {
+		set_err(err, errlen, "null argument or no devices");
+		return DNG_EINVAL;
+	}
+	dng_scan *s = new dng_scan();
+	s->plan = *plan;
+	s->device = devices[0];
+	s->multi = true;
+	for (int k = 0; k < n; k++) {
+		dng_scan *sh = nullptr;
+		int rc = dng_scan_open(plan, devices[k], &sh, err, errlen);
+		if (rc) {
+			dng_scan_destroy(s);
+			return rc;
+		}
+		s->shards.push_back(sh);
+	}
+	*out = s;
+	return DNG_OK;
+}
+
+dng_scan *dng_scan_shard(const dng_scan *s, int i)
+{
+	if (!s || !s->multi || i < 0 || (size_t)i >= s->shards.size())
+		return nullptr;
+	return s->shards[i];
+}
+
+/* what a multi-device scan refuses: not sticky, the scan goes on */
+static int refuse_multi(dng_scan *s, const char *what)
+{
+	if (!s->err_code)
+		s->err = std::string(what) + " on a scan over several devices "
+		    "(it reads files only; per-shard state: dng_scan_shard)";
+	return DNG_EINVAL;
+}
+
 int dng_scan_set_stream(dng_scan *s, void *cuda_stream)
 {
 	if (!s)
 		return DNG_EINVAL;
+	if (s->multi)
+		return refuse_multi(s, "dng_scan_set_stream");
 	if (s->launches || s->bytes_fed)
 		return s->fail(DNG_EINVAL, "dng_scan_set_stream after a feed");
 	s->stream = (cudaStream_t)cuda_stream;
@@ -1035,6 +1083,8 @@ int dng_scan_feed(dng_scan *s, const void *buf, size_t len)
 {
 	if (!s || (!buf && len))
 		return DNG_EINVAL;
+	if (s->multi)
+		return refuse_multi(s, "dng_scan_feed");
 	cudaSetDevice(s->device);
 	if (ensure_ring(s, true))
 		return s->err_code;
@@ -1045,6 +1095,8 @@ int dng_scan_feed_pinned(dng_scan *s, const void *buf, size_t len)
 {
 	if (!s || (!buf && len))
 		return DNG_EINVAL;
+	if (s->multi)
+		return refuse_multi(s, "dng_scan_feed_pinned");
 	cudaSetDevice(s->device);
 	if (ensure_ring(s, false))
 		return s->err_code;
@@ -1106,9 +1158,12 @@ static int feed_fd_sequential(dng_scan *s, int fd, const char *path)
  * pinned buffers (the page cache memcpy is the slow part of reading, so it is
  * spread over cores) while this thread feeds completed blocks, in order, to
  * the H2D ring.  The reference reads with 2 concurrent 16 KB-request streams
- * (lib/datasource-file.js:262-266).
+ * (lib/datasource-file.js:262-266).  Reads bytes [off, off + size) of the
+ * file; `exact`: a file that ends before that fails with DNG_EIO (else it is
+ * read to where it ends now).
  */
-static int feed_file_parallel(dng_scan *s, int fd, size_t size, const char *path)
+static int feed_file_parallel(dng_scan *s, int fd, size_t off, size_t size,
+    const char *path, bool exact)
 {
 	const size_t BLK = (size_t)4 << 20;
 	const size_t NSLOT = 32;	/* 128 MiB of pinned ring */
@@ -1150,15 +1205,18 @@ static int feed_file_parallel(dng_scan *s, int fd, size_t size, const char *path
 			int err = 0;
 			while (have < want) {
 				ssize_t n = pread(fd, dst + have, want - have,
-				    (off_t)(b * BLK + have));
+				    (off_t)(off + b * BLK + have));
 				if (n < 0) {
 					if (errno == EINTR)
 						continue;
 					err = errno;
 					break;
 				}
-				if (n == 0)
-					break;	/* file shrank */
+				if (n == 0) {	/* file shrank */
+					if (exact)
+						err = -1;
+					break;
+				}
 				have += (size_t)n;
 			}
 			std::lock_guard<std::mutex> lk(mu);
@@ -1189,7 +1247,10 @@ static int feed_file_parallel(dng_scan *s, int fd, size_t size, const char *path
 					if (k == 0)
 						rc = s->fail(DNG_EIO,
 						    std::string("read ") + path +
-						    ": " + strerror(read_errno));
+						    ": " + (read_errno < 0 ?
+						    "file is shorter than when "
+						    "it was fed" :
+						    strerror(read_errno)));
 					break;
 				}
 				bytes += (size_t)got[b + k];
@@ -1231,10 +1292,221 @@ static int feed_file_parallel(dng_scan *s, int fd, size_t size, const char *path
 	return rc;
 }
 
+/* ---- scans over several devices (dng_scan_open_devices) -------------------
+ *
+ * The files fed are one logical stream of T bytes, as the reference
+ * concatenates them (CatStreams, lib/datasource-file.js:252-288), so that a
+ * file without a trailing newline joins its last line to the next file's
+ * first.  Shard k of n owns the lines that START in [a_k, a_k+1), a_k =
+ * floor(k T / n): it reads from its first line start to the first line start
+ * at or after a_k+1 (T for the last shard), across file boundaries where its
+ * last line spans them.  Every byte is read by exactly one shard.
+ */
+
+typedef std::pair<std::string, size_t> FedFile;	/* path, size when fed */
+
+static size_t cut_point(size_t T, size_t k, size_t n)
+{
+	return (size_t)((unsigned __int128)T * k / n);
+}
+
+/* a fed file, open for reading, if it still has the size it was fed with */
+static int open_fed(dng_scan *sh, const FedFile &f, int *fd)
+{
+	*fd = open(f.first.c_str(), O_RDONLY);
+	if (*fd < 0)
+		return sh->fail(DNG_EIO, "open " + f.first + ": " +
+		    strerror(errno));
+	struct stat st;
+	if (fstat(*fd, &st) != 0 || (size_t)st.st_size != f.second) {
+		close(*fd);
+		*fd = -1;
+		return sh->fail(DNG_EIO, "read " + f.first + ": file changed "
+		    "size after it was fed");
+	}
+	return 0;
+}
+
+/* the first line start at or after stream position a: a itself when it is 0
+ * or follows a '\n', else just past the next '\n', else T */
+static int line_start(dng_scan *sh, const std::vector<FedFile> &files,
+    size_t T, size_t a, size_t *out)
+{
+	*out = std::min(a, T);
+	if (a == 0 || a >= T)
+		return 0;
+	const size_t pos = a - 1;	/* the byte that decides */
+	std::vector<char> buf((size_t)64 << 10);
+	size_t base = 0;
+	for (const FedFile &f : files) {
+		const size_t end = base + f.second;
+		if (end > pos) {
+			int fd;
+			if (open_fed(sh, f, &fd))
+				return sh->err_code;
+			size_t o = pos > base ? pos - base : 0;
+			while (o < f.second) {
+				ssize_t n = pread(fd, buf.data(), std::min(buf.size(),
+				    f.second - o), (off_t)o);
+				if (n < 0 && errno == EINTR)
+					continue;
+				if (n <= 0) {
+					const std::string why = n < 0 ?
+					    strerror(errno) : "file is shorter "
+					    "than when it was fed";
+					close(fd);
+					return sh->fail(DNG_EIO, "read " + f.first +
+					    ": " + why);
+				}
+				const char *nl = (const char *)memchr(buf.data(),
+				    '\n', (size_t)n);
+				if (nl) {
+					close(fd);
+					*out = base + o + (size_t)(nl - buf.data()) + 1;
+					return 0;
+				}
+				o += (size_t)n;
+			}
+			close(fd);
+		}
+		base = end;
+	}
+	*out = T;
+	return 0;
+}
+
+/* shard k: its byte range of the stream fed to its scan, then its result */
+static int run_shard(dng_scan *s, size_t k, size_t T, dng_result **res)
+{
+	dng_scan *sh = s->shards[k];
+	const size_t n = s->shards.size();
+	cudaSetDevice(sh->device);
+	size_t begin, end;
+	if (line_start(sh, s->files, T, cut_point(T, k, n), &begin) ||
+	    line_start(sh, s->files, T, cut_point(T, k + 1, n), &end))
+		return sh->err_code;
+	size_t base = 0;
+	for (const FedFile &f : s->files) {
+		const size_t lo = std::max(begin, base);
+		const size_t hi = std::min(end, base + f.second);
+		if (lo < hi) {
+			int fd;
+			if (ensure_ring(sh, false) || open_fed(sh, f, &fd))
+				return sh->err_code;
+			int rc = feed_file_parallel(sh, fd, lo - base, hi - lo,
+			    f.first.c_str(), true);
+			close(fd);
+			if (rc)
+				return rc;
+		}
+		base += f.second;
+	}
+	return dng_scan_finish(sh, res);
+}
+
+/* sum values over identical tuples: the host merge of merge.cu */
+static int merge_results(const std::vector<dng_result *> &res,
+    dng_result **out)
+{
+	const size_t n = res.size();
+	std::vector<const void *> bufs(n);
+	std::vector<size_t> lens(n);
+	for (size_t k = 0; k < n; k++)
+		dng_result_dict(res[k], &bufs[k], &lens[k]);
+	void *gdict = nullptr;
+	size_t glen = 0;
+	int rc = dng_dict_union(bufs.data(), lens.data(), n, &gdict, &glen);
+	if (rc)
+		return rc;
+	const size_t G = dng_dict_count(gdict, glen);
+	std::vector<uint64_t> sum(std::max<size_t>(G, 1), 0), one(sum.size());
+	for (size_t k = 0; k < n && !rc; k++) {
+		rc = dng_result_dense(res[k], gdict, glen, one.data(), G);
+		for (size_t i = 0; i < G; i++)
+			sum[i] += one[i];
+	}
+	if (!rc)
+		rc = dng_result_from_dense(res[0], gdict, glen, sum.data(), G, out);
+	dng_buf_free(gdict);
+	return rc;
+}
+
+/* dng_scan_finish of a multi-device scan: one thread per shard */
+static int finish_multi(dng_scan *s, dng_result **out)
+{
+	const size_t n = s->shards.size();
+	size_t T = 0;
+	for (const FedFile &f : s->files)
+		T += f.second;
+	std::vector<dng_result *> res(n, nullptr);
+	std::vector<int> rc(n, 0);
+	const bool again = s->finished;	/* (a second finish reads nothing) */
+	std::vector<std::thread> th;
+	for (size_t k = 0; k < n; k++)
+		th.emplace_back([&, k] {
+			rc[k] = again ? dng_scan_finish(s->shards[k], &res[k]) :
+			    run_shard(s, k, T, &res[k]);
+		});
+	for (auto &t : th)
+		t.join();
+	s->finished = true;
+	int r = 0;
+	for (size_t k = 0; k < n && !r; k++)
+		if (rc[k])
+			r = s->fail(rc[k], "shard " + std::to_string(k) +
+			    " (device " + std::to_string(s->shards[k]->device) +
+			    "): " + s->shards[k]->err);
+	if (!r)
+		r = merge_results(res, out);
+	for (dng_result *x : res)
+		dng_result_destroy(x);
+	return r ? s->fail(r, "merging the shards' results") : DNG_OK;
+}
+
+/* the counters of metric m: the shards' summed */
+static int counters_multi(dng_scan *s, int m, dng_counters *out)
+{
+	memset(out, 0, sizeof (*out));
+	for (dng_scan *sh : s->shards) {
+		dng_counters c;
+		int rc = dng_scan_counters_metric(sh, m, &c);
+		if (rc)
+			return s->fail(rc, sh->err);
+		const uint64_t *a = (const uint64_t *)&c;
+		uint64_t *o = (uint64_t *)out;
+		for (size_t i = 0; i < sizeof (c) / sizeof (uint64_t); i++)
+			o[i] += a[i];
+	}
+	return DNG_OK;
+}
+
+/* dng_scan_feed_file of a multi-device scan: the path and its size only */
+static int record_file(dng_scan *s, const char *path)
+{
+	if (s->err_code)
+		return s->err_code;
+	if (s->finished)
+		return s->fail(DNG_EINVAL, "scan already finished");
+	int fd = open(path, O_RDONLY);
+	if (fd < 0)
+		return s->fail(DNG_EIO, std::string("open ") + path + ": " +
+		    strerror(errno));
+	struct stat st;
+	const bool reg = fstat(fd, &st) == 0 && S_ISREG(st.st_mode);
+	close(fd);
+	if (!reg)
+		return s->fail(DNG_EINVAL, std::string(path) + ": not a regular "
+		    "file (a scan over several devices cuts its input by size)");
+	s->files.emplace_back(path, (size_t)st.st_size);
+	return DNG_OK;
+}
+
 int dng_scan_feed_file(dng_scan *s, const char *path)
 {
 	if (!s || !path)
 		return DNG_EINVAL;
+	if (s->multi)
+		return record_file(s, path);
 	cudaSetDevice(s->device);
 	if (ensure_ring(s, false))
 		return s->err_code;
@@ -1245,7 +1517,7 @@ int dng_scan_feed_file(dng_scan *s, const char *path)
 	struct stat st;
 	int rc;
 	if (fstat(fd, &st) == 0 && S_ISREG(st.st_mode) && st.st_size > 0)
-		rc = feed_file_parallel(s, fd, (size_t)st.st_size, path);
+		rc = feed_file_parallel(s, fd, 0, (size_t)st.st_size, path, false);
 	else
 		rc = feed_fd_sequential(s, fd, path);
 	close(fd);
@@ -1256,6 +1528,8 @@ int dng_scan_feed_device(dng_scan *s, const void *devbuf, size_t len)
 {
 	if (!s || (!devbuf && len))
 		return DNG_EINVAL;
+	if (s->multi)
+		return refuse_multi(s, "dng_scan_feed_device");
 	if (s->err_code)
 		return s->err_code;
 	if (s->finished)
@@ -1379,6 +1653,8 @@ int dng_scan_sync(dng_scan *s)
 {
 	if (!s)
 		return DNG_EINVAL;
+	if (s->multi)	/* (its shards run only inside dng_scan_finish) */
+		return s->err_code;
 	cudaSetDevice(s->device);
 	CK(s, cudaStreamSynchronize(s->copy_stream));
 	CK(s, cudaStreamSynchronize(s->stream));
@@ -1404,6 +1680,8 @@ int dng_scan_counters(dng_scan *s, dng_counters *out)
 {
 	if (!s || !out)
 		return DNG_EINVAL;
+	if (s->multi)
+		return counters_multi(s, 0, out);
 	cudaSetDevice(s->device);
 	if (dng_scan_sync(s))
 		return s->err_code;
@@ -1449,6 +1727,8 @@ int dng_scan_counters_metric(dng_scan *s, int m, dng_counters *out)
 {
 	if (!s || !out || m < 0 || m >= s->plan.dev.nmetrics)
 		return DNG_EINVAL;
+	if (s->multi)
+		return counters_multi(s, m, out);
 	int rc = dng_scan_counters(s, out);
 	if (rc || m == 0)
 		return rc;
@@ -1485,6 +1765,8 @@ int dng_scan_finish(dng_scan *s, dng_result **out)
 		return DNG_EINVAL;
 	if (s->err_code)
 		return s->err_code;
+	if (s->multi)
+		return finish_multi(s, out);
 	cudaSetDevice(s->device);
 	if (flush_tail(s))
 		return s->err_code;
@@ -1570,6 +1852,14 @@ int dng_scan_set_templates(dng_scan *s, int enable)
 {
 	if (!s)
 		return DNG_EINVAL;
+	if (s->multi) {
+		if (s->finished)
+			return s->fail(DNG_EINVAL, "templates are fixed once data "
+			    "has been fed");
+		for (dng_scan *sh : s->shards)
+			dng_scan_set_templates(sh, enable);
+		return DNG_OK;
+	}
 	if (s->tmpl_tried)
 		return s->fail(DNG_EINVAL, "templates are fixed once data has "
 		    "been fed");
@@ -1582,6 +1872,8 @@ int dng_scan_template_stats(dng_scan *s, uint64_t *templates,
 {
 	if (!s)
 		return DNG_EINVAL;
+	if (s->multi)
+		return refuse_multi(s, "dng_scan_template_stats");
 	cudaSetDevice(s->device);
 	if (dng_scan_sync(s))
 		return s->err_code;
@@ -1602,12 +1894,18 @@ int dng_scan_template_stats(dng_scan *s, uint64_t *templates,
 
 uint64_t dng_scan_launch_count(const dng_scan *s)
 {
+	if (s && s->multi) {
+		uint64_t n = 0;
+		for (const dng_scan *sh : s->shards)
+			n += dng_scan_launch_count(sh);
+		return n;
+	}
 	return s ? s->launches + s->aux_launches : 0;
 }
 
 int dng_scan_kernel_kind(const dng_scan *s)
 {
-	if (!s)
+	if (!s || s->multi)
 		return DNG_EINVAL;
 	return kc_pick(s->kc);
 }
@@ -1617,6 +1915,8 @@ int dng_scan_jit_stats(dng_scan *s, int *state, uint64_t *launches,
 {
 	if (!s)
 		return DNG_EINVAL;
+	if (s->multi)
+		return refuse_multi(s, "dng_scan_jit_stats");
 	const int st = s->jit ? s->jit->state.load() : 0;
 	if (state)
 		*state = st;
@@ -1635,6 +1935,8 @@ int dng_scan_kernel_stats(dng_scan *s, double *kernel_ms, uint64_t *launches,
 {
 	if (!s)
 		return DNG_EINVAL;
+	if (s->multi)
+		return refuse_multi(s, "dng_scan_kernel_stats");
 	cudaSetDevice(s->device);
 	if (dng_scan_sync(s))
 		return s->err_code;
@@ -1651,6 +1953,8 @@ int dng_scan_tally_stats(dng_scan *s, uint64_t *inline_overflow, int *f_warps)
 {
 	if (!s)
 		return DNG_EINVAL;
+	if (s->multi)
+		return refuse_multi(s, "dng_scan_tally_stats");
 	cudaSetDevice(s->device);
 	if (dng_scan_sync(s))
 		return s->err_code;
@@ -1692,6 +1996,12 @@ void dng_scan_destroy(dng_scan *s)
 {
 	if (!s)
 		return;
+	if (s->multi) {
+		for (dng_scan *sh : s->shards)
+			dng_scan_destroy(sh);
+		delete s;
+		return;
+	}
 	cudaSetDevice(s->device);
 	if (s->stream)
 		cudaStreamSynchronize(s->stream);

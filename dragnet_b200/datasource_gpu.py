@@ -94,12 +94,18 @@ def stage_counters(plan, c, npoints):
 
 
 def run_plan(plan, files=(), chunks=None, device=0, device_buffers=None,
-             templates=None):
+             templates=None, devices=None):
     """Drive one scan through the C ABI.  Input is any of: files (read by the
-    library), host byte chunks, or (ptr, len) device buffers."""
+    library), host byte chunks, or (ptr, len) device buffers.  devices: more
+    than one device index -> one scan over all of them, the files cut into a
+    byte range per device (files only); its stats are per shard."""
     import json
     p = native.Plan(json.dumps(plan, separators=(',', ':')))
-    s = native.Scan(p, device)
+    multi = devices is not None and len(devices) > 1
+    if devices and not multi:
+        device = devices[0]
+    s = native.Scan(p, devices=list(devices)) if multi else \
+        native.Scan(p, device)
     try:
         if templates is not None:
             s.set_templates(templates)
@@ -111,8 +117,15 @@ def run_plan(plan, files=(), chunks=None, device=0, device_buffers=None,
             s.feed_device(ptr, n)
         res = s.finish()
         flat = s.counters()
-        stats = s.kernel_stats()
-        stats.update(s.template_stats())
+        if multi:
+            stats = {'devices': list(devices), 'shards': []}
+            for sh in s.shards(len(devices)):
+                one = sh.kernel_stats()
+                one.update(sh.template_stats())
+                stats['shards'].append(one)
+        else:
+            stats = s.kernel_stats()
+            stats.update(s.template_stats())
         pts = []
         if 'metrics' in plan:
             # fan-out: points are tagged like the reference tags them
@@ -153,6 +166,9 @@ class DatasourceGpu(object):
         self.ds_indexpath = bc.get('indexPath') or None
         self.ds_filter = dsconfig.get('filter') or None
         self.ds_device = dsconfig.get('device', 0)
+        # a list of device indices, or "all": one scan over all of them
+        # (files cut by bytes, tallies merged exactly), else ds_device alone
+        self.ds_devices = dsconfig.get('devices')
         # (root, timeFormat, after_ms, before_ms) -> [paths]: the reference's
         # own enumeration (lib/datasource-file.js:218-246 findStream), which
         # the real integration keeps; the tests pass their mirror of it
@@ -160,6 +176,11 @@ class DatasourceGpu(object):
 
     def close(self):
         pass
+
+    def _devices(self):
+        if self.ds_devices == 'all':
+            return list(range(native.lib().dng_device_count()))
+        return self.ds_devices
 
     def scan(self, args):
         """lib/datasource-file.js:72-108.  Returns ScanResult or an Error."""
@@ -181,7 +202,8 @@ class DatasourceGpu(object):
         plan = mod_query.scan_plan(query, ds_filter=self.ds_filter,
                                    time_field=self.ds_timefield,
                                    data_format=self.ds_format)
-        return run_plan(plan, files=files, device=self.ds_device)
+        return run_plan(plan, files=files, device=self.ds_device,
+                        devices=self._devices())
 
     def checkTimeArgs(self, args):
         """lib/datasource-file.js:549-556."""
@@ -213,7 +235,8 @@ class DatasourceGpu(object):
             plan = mod_query.scan_plan_multi(
                 queries[base:base + MAX_METRICS], ds_filter=self.ds_filter,
                 time_field=self.ds_timefield, data_format=self.ds_format)
-            r = run_plan(plan, files=files, device=self.ds_device)
+            r = run_plan(plan, files=files, device=self.ds_device,
+                         devices=self._devices())
             for fields, value in r.points:
                 fields[-1] = ('__dn_metric', base + fields[-1][1])
                 pts.append((fields, value))
@@ -353,6 +376,13 @@ def createDatasource(args):
     bc = dsconfig.get('backend_config') or dsconfig
     if not isinstance(bc.get('path'), str):
         return DsError('expected datasource "path" to be a string')
+    devs = dsconfig.get('devices')
+    if devs is not None and devs != 'all' and (
+            not isinstance(devs, (list, tuple)) or not devs or
+            not all(isinstance(d, int) and not isinstance(d, bool) and d >= 0
+                    for d in devs)):
+        return DsError('expected datasource "devices" to be "all" or a '
+                       'non-empty list of device indices')
     return DatasourceGpu(args)
 
 

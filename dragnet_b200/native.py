@@ -58,6 +58,10 @@ _SIGS = [
     ('dng_device_count', ctypes.c_int, []),
     ('dng_scan_open', ctypes.c_int, [_P, ctypes.c_int, ctypes.POINTER(_P),
                                      ctypes.c_char_p, ctypes.c_size_t]),
+    ('dng_scan_open_devices', ctypes.c_int,
+     [_P, ctypes.POINTER(ctypes.c_int), ctypes.c_int, ctypes.POINTER(_P),
+      ctypes.c_char_p, ctypes.c_size_t]),
+    ('dng_scan_shard', _P, [_P, ctypes.c_int]),
     ('dng_scan_set_stream', ctypes.c_int, [_P, _P]),
     ('dng_scan_feed', ctypes.c_int, [_P, _P, ctypes.c_size_t]),
     ('dng_scan_feed_pinned', ctypes.c_int, [_P, _P, ctypes.c_size_t]),
@@ -304,13 +308,64 @@ def dict_union(dicts):
         lib().dng_buf_free(out)
 
 
-class Scan(object):
-    def __init__(self, plan, device=0):
+class _ScanStats(object):
+    """The stats calls of a dng_scan (self.handle)."""
+
+    def kernel_stats(self):
+        ms = ctypes.c_double()
+        n = ctypes.c_uint64()
+        b = ctypes.c_uint64()
+        _check(lib().dng_scan_kernel_stats(self.handle, ctypes.byref(ms),
+                                           ctypes.byref(n), ctypes.byref(b)),
+               self.handle)
+        over = ctypes.c_uint64()
+        fw = ctypes.c_int()
+        _check(lib().dng_scan_tally_stats(self.handle, ctypes.byref(over),
+                                          ctypes.byref(fw)), self.handle)
+        return {'kernel_ms': ms.value, 'launches': int(n.value),
+                'kernel_bytes': int(b.value),
+                'all_launches': int(lib().dng_scan_launch_count(self.handle)),
+                'inline_overflow': int(over.value), 'f_warps': int(fw.value)}
+
+    def template_stats(self):
+        t = ctypes.c_uint64()
+        r = ctypes.c_uint64()
+        _check(lib().dng_scan_template_stats(self.handle, ctypes.byref(t),
+                                             ctypes.byref(r)), self.handle)
+        st = ctypes.c_int()
+        jl = ctypes.c_uint64()
+        cms = ctypes.c_double()
+        lms = ctypes.c_double()
+        err = ctypes.create_string_buffer(512)
+        _check(lib().dng_scan_jit_stats(self.handle, ctypes.byref(st),
+                                        ctypes.byref(jl), ctypes.byref(cms),
+                                        ctypes.byref(lms), err, len(err)),
+               self.handle)
+        kind = lib().dng_scan_kernel_kind(self.handle)
+        return {'templates': int(t.value), 'templated_records': int(r.value),
+                'kernel': {0: 'CTA tiles', 1: 'per-warp chunks',
+                           2: 'F path'}.get(kind, str(kind)),
+                'jit': {'state': int(st.value), 'launches': int(jl.value),
+                        'compile_ms': cms.value, 'link_ms': lms.value,
+                        'error': err.value.decode('utf-8', 'replace')}}
+
+
+class Scan(_ScanStats):
+    def __init__(self, plan, device=0, devices=None):
+        """devices: a list of device indices -> one scan over all of them,
+        the files fed cut into one byte range per device
+        (dng_scan_open_devices; files only)."""
         self.plan = plan
         self.handle = _P()
         err = ctypes.create_string_buffer(512)
-        rc = lib().dng_scan_open(plan.handle, device,
-                                 ctypes.byref(self.handle), err, len(err))
+        if devices is None:
+            rc = lib().dng_scan_open(plan.handle, device,
+                                     ctypes.byref(self.handle), err, len(err))
+        else:
+            devs = (ctypes.c_int * max(len(devices), 1))(*devices)
+            rc = lib().dng_scan_open_devices(plan.handle, devs, len(devices),
+                                             ctypes.byref(self.handle), err,
+                                             len(err))
         if rc != DNG_OK:
             raise DngError(rc, err.value.decode('utf-8', 'replace'))
 
@@ -350,48 +405,14 @@ class Scan(object):
                                               ctypes.byref(c)), self.handle)
         return c.as_dict()
 
-    def kernel_stats(self):
-        ms = ctypes.c_double()
-        n = ctypes.c_uint64()
-        b = ctypes.c_uint64()
-        _check(lib().dng_scan_kernel_stats(self.handle, ctypes.byref(ms),
-                                           ctypes.byref(n), ctypes.byref(b)),
-               self.handle)
-        over = ctypes.c_uint64()
-        fw = ctypes.c_int()
-        _check(lib().dng_scan_tally_stats(self.handle, ctypes.byref(over),
-                                          ctypes.byref(fw)), self.handle)
-        return {'kernel_ms': ms.value, 'launches': int(n.value),
-                'kernel_bytes': int(b.value),
-                'all_launches': int(lib().dng_scan_launch_count(self.handle)),
-                'inline_overflow': int(over.value), 'f_warps': int(fw.value)}
-
     def set_templates(self, enable):
         """Record templates on/off (default on); before the first feed."""
         _check(lib().dng_scan_set_templates(self.handle, 1 if enable else 0),
                self.handle)
 
-    def template_stats(self):
-        t = ctypes.c_uint64()
-        r = ctypes.c_uint64()
-        _check(lib().dng_scan_template_stats(self.handle, ctypes.byref(t),
-                                             ctypes.byref(r)), self.handle)
-        st = ctypes.c_int()
-        jl = ctypes.c_uint64()
-        cms = ctypes.c_double()
-        lms = ctypes.c_double()
-        err = ctypes.create_string_buffer(512)
-        _check(lib().dng_scan_jit_stats(self.handle, ctypes.byref(st),
-                                        ctypes.byref(jl), ctypes.byref(cms),
-                                        ctypes.byref(lms), err, len(err)),
-               self.handle)
-        kind = lib().dng_scan_kernel_kind(self.handle)
-        return {'templates': int(t.value), 'templated_records': int(r.value),
-                'kernel': {0: 'CTA tiles', 1: 'per-warp chunks',
-                           2: 'F path'}.get(kind, str(kind)),
-                'jit': {'state': int(st.value), 'launches': int(jl.value),
-                        'compile_ms': cms.value, 'link_ms': lms.value,
-                        'error': err.value.decode('utf-8', 'replace')}}
+    def shards(self, n):
+        """The n shards of a multi-device scan."""
+        return [Shard(self, i) for i in range(n)]
 
     def close(self):
         if self.handle:
@@ -404,6 +425,16 @@ class Scan(object):
             self.close()
         except Exception:
             pass
+
+
+class Shard(_ScanStats):
+    """Shard i of a multi-device Scan: its stats only (dng_scan_shard)."""
+
+    def __init__(self, scan, i):
+        self.scan = scan                # the owner outlives this view
+        self.handle = lib().dng_scan_shard(scan.handle, i)
+        if not self.handle:
+            raise DngError(-1, 'no shard %d' % i)
 
 
 def gen_params(seed=0xD5A60000, total_records=1000, string_latency=False,

@@ -106,6 +106,41 @@ int dng_device_count(void);
 int dng_scan_open(const dng_plan *plan, int device, dng_scan **out,
     char *err, size_t errlen);
 
+/*
+ * One scan over several devices, for files only.  The files fed are one
+ * logical byte stream of T bytes (their sizes taken when fed), as the
+ * reference concatenates them: a file without a trailing newline joins its
+ * last line to the next file's first.  dng_scan_finish cuts that stream into
+ * n shards, shard k owning the lines that start in [floor(k T/n),
+ * floor((k+1) T/n)), and scans each with an ordinary scan of its own on
+ * devices[k], from a thread of its own; the points and counters it returns
+ * are exactly those of one scan of the same files (counters summed per
+ * metric; the shards' `bytes` sum to T).
+ *   - A device may be listed more than once; a bad index fails here with
+ *     DNG_ENODEV, as dng_scan_open does, as does a machine without CUDA.
+ *   - dng_scan_feed_file only records the path and its size: it must name a
+ *     regular file, and one whose size has changed by the time it is read
+ *     fails the scan with DNG_EIO.  The 16 MiB line limit holds across cuts.
+ *   - dng_scan_feed, _pinned, _device and dng_scan_set_stream return
+ *     DNG_EINVAL; set_templates applies to every shard.
+ *   - Each shard holds what a single scan holds: its device buffers, a
+ *     128 MiB pinned file ring and, while it reads, DNG_READ_THREADS
+ *     reader threads (default 16) -- the knob is per shard, so n shards
+ *     read with up to 16 n threads.
+ */
+int dng_scan_open_devices(const dng_plan *plan, const int *devices, int n,
+    dng_scan **out, char *err, size_t errlen);
+/*
+ * Shard i of a scan from dng_scan_open_devices (NULL for any other scan or
+ * index), owned by that scan: for the stats calls only (kernel_kind,
+ * kernel_stats, tally_stats, template_stats, jit_stats, launch_count, and
+ * counters after finish); never feed, finish or destroy it.  Shards learn
+ * their templates from their own head and may pick different kernels;
+ * results never depend on either.  Those stats calls on the multi-device scan
+ * itself return DNG_EINVAL (dng_scan_launch_count sums the shards').
+ */
+dng_scan *dng_scan_shard(const dng_scan *scan, int i);
+
 /* Run this scan's kernels on a caller-owned CUDA stream (a cudaStream_t) instead
  * of the scan's private one, e.g. to bracket them with the caller's events.
  * Call before the first feed. */

@@ -6,6 +6,10 @@
  *
  *   scanOpen(planJson, device, breakdownNames[, tagMetric])
  *                               -> scan object (throws Error on DNG_E*)
+ *                                  device: an index, an array of them or
+ *                                  "all" (every device): with more than
+ *                                  one, one scan over all of them
+ *                                  (dng_scan_open_devices), fed files only
  *                                  For a fan-out plan ("metrics": [...], the
  *                                  scan of `dn build`), breakdownNames holds
  *                                  every metric's names one metric after the
@@ -314,7 +318,29 @@ napi_value ScanOpen(napi_env env, napi_callback_info info)
 	}
 	const std::string plan = GetString(env, argv[0]);
 	int32_t device = 0;
-	napi_get_value_int32(env, argv[1], &device);
+	std::vector<int> devices;
+	uint32_t ndev = 0;
+	char all[4] = "";
+	size_t alllen = 0;
+	const bool listed = napi_get_array_length(env, argv[1], &ndev) ==
+	    napi_ok;
+	if (listed) {
+		for (uint32_t i = 0; i < ndev; i++) {
+			napi_value e;
+			int32_t d = -1;
+			napi_get_element(env, argv[1], i, &e);
+			napi_get_value_int32(env, e, &d);
+			devices.push_back(d);
+		}
+	} else if (napi_get_value_string_utf8(env, argv[1], all, sizeof (all),
+	    &alllen) == napi_ok && strcmp(all, "all") == 0) {
+		for (int d = 0; d < dng_device_count(); d++)
+			devices.push_back(d);
+	} else {
+		napi_get_value_int32(env, argv[1], &device);
+	}
+	if (devices.size() == 1)
+		device = devices[0];
 	ScanWrap *w = new ScanWrap();
 	uint32_t nnames = 0;
 	napi_get_array_length(env, argv[2], &nnames);
@@ -330,7 +356,12 @@ napi_value ScanOpen(napi_env env, napi_callback_info info)
 	char err[512];
 	err[0] = '\0';
 	int rc = dng_plan_create(plan.c_str(), &w->plan, err, sizeof (err));
-	if (rc == 0)
+	/* (an empty list is refused there; "all" without devices fails as
+	 * dng_scan_open does) */
+	if (rc == 0 && (devices.size() > 1 || (listed && devices.empty())))
+		rc = dng_scan_open_devices(w->plan, devices.data(),
+		    (int)devices.size(), &w->scan, err, sizeof (err));
+	else if (rc == 0)
 		rc = dng_scan_open(w->plan, device, &w->scan, err, sizeof (err));
 	if (rc != 0) {
 		Release(w);

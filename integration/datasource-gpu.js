@@ -48,6 +48,13 @@ function DatasourceGpu(args, fileds)
 	this.ds_timefield = args.dsconfig.ds_backend_config.timeField || null;
 	this.ds_filter = args.dsconfig.ds_filter || null;
 	this.ds_device = args.dsconfig.ds_backend_config.device || 0;
+	/*
+	 * "devices": an array of device indices or "all": one scan over all of
+	 * them, the files cut into one byte range per device and the tallies
+	 * merged exactly (dng_scan_open_devices); without it, "device" alone.
+	 */
+	if (args.dsconfig.ds_backend_config.devices !== undefined)
+		this.ds_device = args.dsconfig.ds_backend_config.devices;
 	this.ds_log = args.log;
 }
 
