@@ -32,6 +32,7 @@
 #include "scan_kernel.cuh"
 #include "fast_kernel.cuh"
 #include "jit.h"
+#include "jit_cache.h"
 #include "gen.cuh"
 
 using namespace dng;
@@ -1971,6 +1972,29 @@ int dng_scan_tally_stats(dng_scan *s, uint64_t *inline_overflow, int *f_warps)
 void dng_jit_finish(void)
 {
 	dng::jit_finish();
+}
+
+int dng_jit_cache_dir(const char *dir)
+{
+	dng::jit_cache_set_dir(dir);
+	return DNG_OK;
+}
+
+int dng_jit_cache_stats(uint64_t *hits, uint64_t *misses, uint64_t *writes,
+    uint64_t *evictions, uint64_t *errors)
+{
+	const dng::JitCacheStats st = dng::jit_cache_stats();
+	if (hits)
+		*hits = st.hits;
+	if (misses)
+		*misses = st.misses;
+	if (writes)
+		*writes = st.writes;
+	if (evictions)
+		*evictions = st.evictions;
+	if (errors)
+		*errors = st.errors;
+	return DNG_OK;
 }
 
 void dng_release_cached(void)

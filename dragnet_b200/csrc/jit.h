@@ -16,8 +16,10 @@
  *
  * Kernels are cached per process by what the generated source and its build
  * are made from (jit_key), so a scan whose kernel is cached generates no
- * source.  Both libraries are dlopen()ed; without them (or with DNG_JIT=0)
- * scans use the interpreted matcher.
+ * source; with a cache directory also on disk (jit_cache.h), so that a new
+ * process loads the kernel an earlier one linked.  Both libraries are
+ * dlopen()ed; without them (or with DNG_JIT=0) scans use the interpreted
+ * matcher.
  */
 #ifndef DNG_JIT_H
 #define DNG_JIT_H
@@ -36,6 +38,7 @@ struct JitKernels {
 	cudaLibrary_t lib = nullptr;
 	cudaKernel_t kern = nullptr;	/* dng_scan_kernel_j for one slice size */
 	std::atomic<int> state{0};	/* 0 being built, 1 ready, 2 failed */
+	bool disk_pending = false;	/* being looked up on disk (jit_cache.h) */
 	bool ok = false;
 	std::string err;
 	double compile_ms = 0, link_ms = 0;
@@ -61,10 +64,14 @@ std::string jit_key(const u8 *blob, size_t bytes, const FPlan *plan, int nsl,
     int dev, int smem_max);
 
 /*
- * The kernels for this blob and plan on device `dev`, from the cache, or built
- * now from jit_source(blob, bytes, plan): on the caller's thread if `wait`
- * (then state is 1 or 2 on return), else on a worker thread (state 0 until it
- * is done: the caller keeps using the interpreted matcher meanwhile).
+ * The kernels for this blob and plan on device `dev`, from the cache, else
+ * from the cache directory (loaded on the caller's thread: state 1 on return,
+ * in either mode), or built now from jit_source(blob, bytes, plan): on the
+ * caller's thread if `wait` (then state is 1 or 2 on return), else on a
+ * worker thread (state 0 until it is done: the caller keeps using the
+ * interpreted matcher meanwhile).  A build is written to the cache directory
+ * after the kernel is ready, never on the caller's thread: by the worker that
+ * built it, or (wait) by a thread of its own, joined like the workers.
  * smem_max = dynamic shared memory the kernels may be launched with.
  */
 std::shared_ptr<JitKernels> jit_request(const u8 *blob, size_t bytes,

@@ -1,7 +1,7 @@
 /*
  * jit_load.cpp: the per-process cache of run-time compiled kernels (jit.h),
- * their compilation off the caller's thread and their loading into the CUDA
- * runtime.
+ * the kernels kept on disk (jit_cache.h), their compilation off the caller's
+ * thread and their loading into the CUDA runtime.
  */
 #include <stdlib.h>
 
@@ -12,6 +12,7 @@
 #include <vector>
 
 #include "jit.h"
+#include "jit_cache.h"
 
 namespace dng {
 
@@ -57,8 +58,62 @@ void join_workers_at_exit()
 	g_workers.join_all();
 }
 
+/* the linked kernel in `cubin` loaded for device `dev` (current on this
+ * thread then) */
+bool load_into(JitKernels &k, const std::string &cubin, int dev, int smem_max,
+    std::string &err)
+{
+	cudaSetDevice(dev);
+	/* (an error some earlier call left for its caller's check stays) */
+	const bool clean = cudaPeekAtLastError() == cudaSuccess;
+	cudaError_t e = cudaLibraryLoadData(&k.lib, cubin.data(), nullptr,
+	    nullptr, 0, nullptr, nullptr, 0);
+	if (e == cudaSuccess)
+		e = cudaLibraryGetKernel(&k.kern, k.lib, "dng_scan_kernel_j");
+	if (e == cudaSuccess)
+		e = cudaFuncSetAttribute((const void *)k.kern,
+		    cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max);
+	if (e != cudaSuccess) {
+		/* (ours is not left for the scan's next error check to find) */
+		if (clean)
+			cudaGetLastError();
+		if (k.lib)
+			cudaLibraryUnload(k.lib);
+		k.lib = nullptr;
+		k.kern = nullptr;
+		err = std::string("loading the linked kernel: ") +
+		    cudaGetErrorString(e);
+		return false;
+	}
+	return true;
+}
+
+/* where a kernel goes on disk: the cache directory ("" none), the entry's key
+ * and its file name */
+struct DiskEntry {
+	std::string dir, key, name;
+};
+
+/*
+ * The key of a kernel on disk: jit_key() with the device's compute capability
+ * in place of its index (an index means nothing to another process), after
+ * the build id of this library file; "" (no cache) if that cannot be read.
+ */
+std::string disk_key(const u8 *blob, size_t bytes, const FPlan *plan, int nsl,
+    int dev, int smem_max)
+{
+	static const std::string build = jit_cache_build_id(nullptr);
+	if (build.empty())
+		return "";
+	int major = 0, minor = 0;
+	cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
+	cudaDeviceGetAttribute(&minor, cudaDevAttrComputeCapabilityMinor, dev);
+	return build + jit_key(blob, bytes, plan, nsl, major * 10 + minor,
+	    smem_max);
+}
+
 void build_into(std::shared_ptr<JitKernels> k, std::string source, int nsl,
-    int dev, int smem_max, std::string key)
+    int dev, int smem_max, std::string key, DiskEntry disk, bool on_caller)
 {
 	/* one build at a time; by the time it is this one's turn the scan that
 	 * asked may be gone (short scans, test suites), or the process on its
@@ -81,21 +136,8 @@ void build_into(std::shared_ptr<JitKernels> k, std::string source, int nsl,
 	}
 	std::string cubin, err;
 	bool ok = jit_build(source, nsl, cubin, err, &k->compile_ms, &k->link_ms);
-	if (ok) {
-		cudaSetDevice(dev);
-		cudaError_t e = cudaLibraryLoadData(&k->lib, cubin.data(), nullptr,
-		    nullptr, 0, nullptr, nullptr, 0);
-		if (e == cudaSuccess)
-			e = cudaLibraryGetKernel(&k->kern, k->lib, "dng_scan_kernel_j");
-		if (e == cudaSuccess)
-			e = cudaFuncSetAttribute((const void *)k->kern,
-			    cudaFuncAttributeMaxDynamicSharedMemorySize, smem_max);
-		if (e != cudaSuccess) {
-			ok = false;
-			err = std::string("loading the linked kernel: ") +
-			    cudaGetErrorString(e);
-		}
-	}
+	if (ok)
+		ok = load_into(*k, cubin, dev, smem_max, err);
 	{
 		std::lock_guard<std::mutex> g(g_mu);
 		k->err = err;
@@ -103,6 +145,20 @@ void build_into(std::shared_ptr<JitKernels> k, std::string source, int nsl,
 		k->state.store(ok ? 1 : 2);
 	}
 	g_cv.notify_all();
+	/* written after the scan has its kernel, and never on the scan's
+	 * thread: a build that ran there (sync mode) hands the write to a
+	 * thread of its own, joined with the compiler threads */
+	if (!ok || disk.dir.empty())
+		return;
+	if (!on_caller) {
+		jit_cache_put(disk.dir, disk.name, disk.key, cubin,
+		    JIT_CACHE_BOUND);
+		return;
+	}
+	std::lock_guard<std::mutex> g(g_mu);
+	if (!g_exiting)
+		g_workers.th.emplace_back(jit_cache_put, disk.dir, disk.name,
+		    disk.key, std::move(cubin), JIT_CACHE_BOUND);
 }
 
 } /* namespace */
@@ -125,10 +181,49 @@ std::shared_ptr<JitKernels> jit_request(const u8 *blob, size_t bytes,
 		/* (failures are cached too: not tried again for every scan) */
 		k = std::make_shared<JitKernels>();
 		g_cache[key] = k;
+		/* a kernel on disk is loaded here, on the caller's thread, in
+		 * either mode: the scan's first launch runs it, and neither
+		 * compiler library is loaded.  Requests for it meanwhile
+		 * (the shards of a multi-device scan) wait for the answer */
+		DiskEntry disk;
+		disk.dir = jit_cache_dir();
+		k->disk_pending = !disk.dir.empty();
 		g.unlock();
+		if (!disk.dir.empty()) {
+			disk.key = disk_key(blob, bytes, plan, nsl, dev, smem_max);
+			disk.name = jit_cache_name(disk.key);
+			std::string cubin, err;
+			if (disk.key.empty()) {
+				/* (no build id: nothing read or written) */
+				jit_cache_count_error();
+				disk.dir.clear();
+			} else if (jit_cache_get(disk.dir, disk.name, disk.key,
+			    cubin)) {
+				int cur = dev;
+				cudaGetDevice(&cur);
+				const bool ok = load_into(*k, cubin, dev, smem_max,
+				    err);
+				cudaSetDevice(cur);
+				if (ok) {
+					g.lock();
+					k->ok = true;
+					k->state.store(1);
+					k->disk_pending = false;
+					g_cv.notify_all();
+					return k;
+				}
+				/* (a cubin the driver refuses: built anew) */
+				jit_cache_count_error();
+			}
+			g.lock();
+			k->disk_pending = false;
+			g_cv.notify_all();
+			g.unlock();
+		}
 		const std::string source = jit_source(blob, bytes, plan);
 		if (wait) {
-			build_into(k, source, nsl, dev, smem_max, key);
+			build_into(k, source, nsl, dev, smem_max, key, disk,
+			    true);
 			g.lock();
 		} else {
 			/* (the libraries loaded and run once, here, and then
@@ -138,11 +233,13 @@ std::shared_ptr<JitKernels> jit_request(const u8 *blob, size_t bytes,
 			std::call_once(once, [] { atexit(join_workers_at_exit); });
 			g.lock();
 			g_workers.th.emplace_back(build_into, k, source, nsl, dev,
-			    smem_max, key);
+			    smem_max, key, disk, false);
 		}
 	}
 	if (wait)
 		g_cv.wait(g, [&] { return k->state.load() != 0; });
+	else
+		g_cv.wait(g, [&] { return !k->disk_pending; });
 	return k;
 }
 

@@ -76,6 +76,9 @@ _SIGS = [
     ('dng_scan_destroy', None, [_P]),
     ('dng_release_cached', None, []),
     ('dng_jit_finish', None, []),
+    ('dng_jit_cache_dir', ctypes.c_int, [ctypes.c_char_p]),
+    ('dng_jit_cache_stats', ctypes.c_int,
+     [ctypes.POINTER(ctypes.c_uint64)] * 5),
     ('dng_scan_kernel_stats', ctypes.c_int,
      [_P, ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_uint64),
       ctypes.POINTER(ctypes.c_uint64)]),
@@ -161,6 +164,26 @@ def lib():
         # tear themselves down at exit() can crash the process
         atexit.register(L.dng_jit_finish)
     return _lib
+
+
+JIT_CACHE_STATS = ['hits', 'misses', 'writes', 'evictions', 'errors']
+
+
+def set_jit_cache_dir(path):
+    """Keep the run-time compiled kernels of this process's scans in
+    directory `path` (None: no cache), so that later processes load them
+    instead of building them (dng_jit_cache_dir; overrides the environment's
+    DNG_JIT_CACHE_DIR).  Before the first scan is opened."""
+    _check(lib().dng_jit_cache_dir(None if path is None
+                                   else os.fsencode(path)))
+
+
+def jit_cache_stats():
+    """The process's counters of that cache: {hits, misses, writes,
+    evictions, errors}."""
+    v = [ctypes.c_uint64() for _ in JIT_CACHE_STATS]
+    _check(lib().dng_jit_cache_stats(*[ctypes.byref(x) for x in v]))
+    return {n: int(x.value) for n, x in zip(JIT_CACHE_STATS, v)}
 
 
 def _check(rc, scan=None, msg=None):

@@ -184,6 +184,33 @@ void dng_release_cached(void);
  * exit() tears the compiler libraries down can crash the process.  The Python
  * package calls it from an atexit handler. */
 void dng_jit_finish(void);
+/*
+ * Keeps the F path's run-time compiled kernels (dng_scan_jit_stats) in `dir`,
+ * one file per kernel, so that a later process loads the kernel instead of
+ * compiling and linking it, and runs it from its first launch in
+ * DNG_JIT=async mode too.  NULL or "" turns the cache off for this process.
+ * Overrides the environment's DNG_JIT_CACHE_DIR; call it before the first scan
+ * is opened.  Off by default: then nothing is read or written.
+ *
+ * An entry is found by its full key: the scan's templates and plan, the lane
+ * slice size, the shared-memory limit, the device's compute capability and a
+ * build id of this library (a hash of the whole library file), so a kernel is
+ * only ever loaded by the same library file that linked it.  A damaged,
+ * truncated or foreign entry is a miss and the kernel is linked again; the
+ * directory (created with mode 0700) is held under 512 MiB by deleting the
+ * least recently used entries.  A directory that is not the calling user's,
+ * or that group or others may write to, is not used (an error is counted):
+ * whoever can write an entry chooses the code a scan runs.  No cache failure
+ * fails a scan or changes its results: it is counted and the kernel is built
+ * as without the cache.
+ */
+int dng_jit_cache_dir(const char *dir);
+/* process-wide counters of that cache: entries loaded, looked up and not
+ * found (or damaged), written, deleted to stay under the bound, and failures
+ * (a directory that cannot be created or written, an entry the driver
+ * refused); any pointer may be NULL */
+int dng_jit_cache_stats(uint64_t *hits, uint64_t *misses, uint64_t *writes,
+    uint64_t *evictions, uint64_t *errors);
 
 /* Device time (ms, CUDA events on the scan stream) spent in scan kernels and
  * the number of kernel launches since open; for bench.py's roofline. */

@@ -23,6 +23,9 @@
  *                                  (counters: of the plan's first metric)
  *                                  counters = {lines, invalid_json, ...}
  *   scan.close()                   dng_scan_destroy + dng_plan_destroy
+ *   jitCacheDir(dir)               dng_jit_cache_dir: keep the compiled scan
+ *                                  kernels in directory `dir` (null: none)
+ *                                  for later processes; before scanOpen
  *
  * Every call that can block (reads, H2D copies, waiting for kernels) runs as
  * napi async work on the libuv pool: the event loop is never blocked, as the
@@ -382,6 +385,28 @@ napi_value ScanOpen(napi_env env, napi_callback_info info)
 	return obj;
 }
 
+/* jitCacheDir(dir): a string, or null / undefined for none */
+napi_value JitCacheDir(napi_env env, napi_callback_info info)
+{
+	size_t argc = 1;
+	napi_value argv[1], undef;
+	napi_get_undefined(env, &undef);
+	if (napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr) !=
+	    napi_ok) {
+		Throw(env, "jitCacheDir(dir)");
+		return nullptr;
+	}
+	size_t n = 0;
+	const bool named = argc >= 1 && napi_get_value_string_utf8(env, argv[0],
+	    nullptr, 0, &n) == napi_ok;
+	const std::string dir = named ? GetString(env, argv[0]) : std::string();
+	if (dng_jit_cache_dir(named ? dir.c_str() : nullptr) != 0) {
+		Throw(env, "dragnet_gpu: jitCacheDir failed");
+		return nullptr;
+	}
+	return undef;
+}
+
 } /* namespace */
 
 NAPI_MODULE_INIT()
@@ -390,5 +415,8 @@ NAPI_MODULE_INIT()
 	napi_create_function(env, "scanOpen", NAPI_AUTO_LENGTH, ScanOpen, nullptr,
 	    &fn);
 	napi_set_named_property(env, exports, "scanOpen", fn);
+	napi_create_function(env, "jitCacheDir", NAPI_AUTO_LENGTH, JitCacheDir,
+	    nullptr, &fn);
+	napi_set_named_property(env, exports, "jitCacheDir", fn);
 	return exports;
 }

@@ -11,6 +11,12 @@
  *
  *     if (bename == 'gpu')
  *             return (mod_datasource_gpu.createDatasource(args));
+ *
+ * A host that keeps a directory for compiled scan kernels passes it as
+ * args.jitCacheDir, next to log and dsconfig: later `dn` processes then load
+ * the kernels instead of compiling them (dng_jit_cache_dir).  It is a setting
+ * of the process, not of a datasource, so the first datasource created sets
+ * it; without it the environment's DNG_JIT_CACHE_DIR applies.
  */
 
 var mod_assertplus = require('assert-plus');
@@ -22,14 +28,22 @@ var VError = require('verror');
 var mod_datasource_file = require('./datasource-file');
 var mod_dragnet_impl = require('./dragnet-impl');
 var dragnet_gpu = require('dragnet_gpu');	/* the N-API addon */
+var jitCacheDirSet = false;
 
 exports.createDatasource = function createDatasource(args)
 {
 	var filecfg, fileds;
 
 	mod_assertplus.object(args.dsconfig);
+	mod_assertplus.optionalString(args.jitCacheDir, 'args.jitCacheDir');
 	if (typeof (args.dsconfig.ds_backend_config.path) != 'string')
 		return (new VError('expected datasource "path" to be a string'));
+
+	/* (before the first scan is opened) */
+	if (args.jitCacheDir !== undefined && !jitCacheDirSet) {
+		dragnet_gpu.jitCacheDir(args.jitCacheDir);
+		jitCacheDirSet = true;
+	}
 
 	/* query/indexRead and the index files stay on the file backend */
 	filecfg = Object.create(args.dsconfig);
