@@ -34,6 +34,7 @@
 #include "jit.h"
 #include "jit_cache.h"
 #include "gen.cuh"
+#include "direct_read.h"
 
 using namespace dng;
 
@@ -170,6 +171,9 @@ struct dng_scan {
 	/* pinned block ring of dng_scan_feed_file's reader threads */
 	u8 *file_buf = nullptr;
 	cudaEvent_t file_done[32] = {};
+	/* dng_scan_read_stats */
+	uint64_t direct_bytes = 0, buffered_bytes = 0, direct_ranges = 0;
+	uint64_t read_fallbacks = 0;
 	/* stats */
 	std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_pairs;
 	std::vector<cudaEvent_t> ev_pool;
@@ -1155,18 +1159,22 @@ static int feed_fd_sequential(dng_scan *s, int fd, const char *path)
 }
 
 /*
- * Regular files: a few reader threads pread() fixed-size blocks into a ring of
- * pinned buffers (the page cache memcpy is the slow part of reading, so it is
- * spread over cores) while this thread feeds completed blocks, in order, to
- * the H2D ring.  The reference reads with 2 concurrent 16 KB-request streams
+ * Regular files: a few reader threads read fixed-size blocks into a ring of
+ * pinned buffers while this thread feeds completed blocks, in order, to the
+ * H2D ring.  The reference reads with 2 concurrent 16 KB-request streams
  * (lib/datasource-file.js:262-266).  Reads bytes [off, off + size) of the
  * file; `exact`: a file that ends before that fails with DNG_EIO (else it is
  * read to where it ends now).
+ *
+ * A range mostly absent from the page cache is read with O_DIRECT, storage
+ * straight into the pinned ring (direct_read.h); a cached one with pread,
+ * whose page-cache memcpy is the slow part of reading, so it is spread over
+ * the threads.
  */
 static int feed_file_parallel(dng_scan *s, int fd, size_t off, size_t size,
     const char *path, bool exact)
 {
-	const size_t BLK = (size_t)4 << 20;
+	const size_t BLK = DR_BLK;
 	const size_t NSLOT = 32;	/* 128 MiB of pinned ring */
 	const size_t LAG = 6;		/* blocks kept back for in-flight DMA */
 	const size_t GROUP = 4;		/* ready neighbours fed as one chunk */
@@ -1176,8 +1184,27 @@ static int feed_file_parallel(dng_scan *s, int fd, size_t off, size_t size,
 			CK(s, cudaEventCreateWithFlags(&s->file_done[i],
 			    cudaEventDisableTiming));
 	}
-	const size_t nblocks = (size + BLK - 1) / BLK;
-	/* 16 readers by default: more threads contend in the page cache */
+	DrRange r;
+	r.fd = fd;
+	r.exact = exact;
+	size_t align = 1;
+	if (dr_direct(dr_cached_fraction(fd, off, size))) {
+		/* the same file, whatever happened to the path since */
+		const std::string self = "/proc/self/fd/" + std::to_string(fd);
+		align = dr_direct_align(dr_align(fd), s->file_buf);
+		if (align)
+			r.dfd = open(self.c_str(), O_RDONLY | O_DIRECT);
+		if (r.dfd >= 0) {
+			r.direct = true;
+		} else {
+			s->read_fallbacks++;
+			align = 1;
+		}
+	}
+	r.plan = dr_plan(off, size, align);
+	const size_t nblocks = r.plan.nblocks;
+	/* 16 readers by default: more threads contend in the page cache, and
+	 * 16 direct reads in flight are the storage's queue depth */
 	size_t nthreads = env_size("DNG_READ_THREADS", 16);
 	nthreads = std::max<size_t>(1, std::min(nthreads, std::min(nblocks,
 	    NSLOT - LAG)));
@@ -1185,7 +1212,7 @@ static int feed_file_parallel(dng_scan *s, int fd, size_t off, size_t size,
 	std::condition_variable cv;
 	size_t next_block = 0;		/* next block a reader takes */
 	size_t released = NSLOT;	/* blocks < released may be (re)filled */
-	std::vector<ssize_t> got(nblocks, -2);	/* -2 pending, -1 error */
+	std::vector<ssize_t> got(nblocks, -2);	/* fed bytes; -2 pending, -1 error */
 	int read_errno = 0;
 	bool abort_all = false;
 	auto reader = [&]() {
@@ -1201,31 +1228,18 @@ static int feed_file_parallel(dng_scan *s, int fd, size_t off, size_t size,
 				if (abort_all)
 					return;
 			}
-			size_t want = std::min(BLK, size - b * BLK), have = 0;
-			u8 *dst = s->file_buf + (b % NSLOT) * BLK;
-			int err = 0;
-			while (have < want) {
-				ssize_t n = pread(fd, dst + have, want - have,
-				    (off_t)(off + b * BLK + have));
-				if (n < 0) {
-					if (errno == EINTR)
-						continue;
-					err = errno;
-					break;
-				}
-				if (n == 0) {	/* file shrank */
-					if (exact)
-						err = -1;
-					break;
-				}
-				have += (size_t)n;
-			}
+			size_t lo = 0, hi = 0;
+			bool via_direct = false;
+			int err = dr_fetch(pread, r, b,
+			    s->file_buf + (b % NSLOT) * BLK, &lo, &hi, &via_direct);
 			std::lock_guard<std::mutex> lk(mu);
 			if (err) {
 				read_errno = err;
 				got[b] = -1;
 			} else {
-				got[b] = (ssize_t)have;
+				got[b] = (ssize_t)(hi - lo);
+				(via_direct ? s->direct_bytes : s->buffered_bytes) +=
+				    hi - lo;
 			}
 			cv.notify_all();
 		}
@@ -1256,15 +1270,16 @@ static int feed_file_parallel(dng_scan *s, int fd, size_t off, size_t size,
 				}
 				bytes += (size_t)got[b + k];
 				k++;
-				if ((size_t)got[b + k - 1] != BLK)
+				if (r.plan.lo(b + k - 1) + (size_t)got[b + k - 1]
+				    != BLK)
 					break;	/* short block: last one */
 			}
 		}
 		if (rc)
 			break;
 		if (bytes)
-			rc = feed_host(s, s->file_buf + (b % NSLOT) * BLK, bytes,
-			    true);
+			rc = feed_host(s, s->file_buf + (b % NSLOT) * BLK +
+			    r.plan.lo(b), bytes, true);
 		for (size_t j = 0; j < k && !rc; j++)
 			rc = s->cuda(cudaEventRecord(
 			    s->file_done[(b + j) % NSLOT], s->copy_stream),
@@ -1288,6 +1303,10 @@ static int feed_file_parallel(dng_scan *s, int fd, size_t off, size_t size,
 	}
 	for (auto &t : pool)
 		t.join();
+	if (r.dfd >= 0)
+		close(r.dfd);
+	s->direct_ranges += r.direct;	/* (not when it fell back) */
+	s->read_fallbacks += r.fallbacks;
 	/* the pinned ring is reused by the next file: drain its copies */
 	cudaStreamSynchronize(s->copy_stream);
 	return rc;
@@ -1902,6 +1921,30 @@ uint64_t dng_scan_launch_count(const dng_scan *s)
 		return n;
 	}
 	return s ? s->launches + s->aux_launches : 0;
+}
+
+int dng_scan_read_stats(dng_scan *s, uint64_t *direct_bytes,
+    uint64_t *buffered_bytes, uint64_t *direct_ranges, uint64_t *fallbacks)
+{
+	if (!s)
+		return DNG_EINVAL;
+	uint64_t v[4] = { s->direct_bytes, s->buffered_bytes, s->direct_ranges,
+	    s->read_fallbacks };
+	for (dng_scan *sh : s->shards) {
+		uint64_t one[4];
+		dng_scan_read_stats(sh, &one[0], &one[1], &one[2], &one[3]);
+		for (int i = 0; i < 4; i++)
+			v[i] += one[i];
+	}
+	if (direct_bytes)
+		*direct_bytes = v[0];
+	if (buffered_bytes)
+		*buffered_bytes = v[1];
+	if (direct_ranges)
+		*direct_ranges = v[2];
+	if (fallbacks)
+		*fallbacks = v[3];
+	return DNG_OK;
 }
 
 int dng_scan_kernel_kind(const dng_scan *s)

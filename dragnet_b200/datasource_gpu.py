@@ -122,10 +122,12 @@ def run_plan(plan, files=(), chunks=None, device=0, device_buffers=None,
             for sh in s.shards(len(devices)):
                 one = sh.kernel_stats()
                 one.update(sh.template_stats())
+                one.update(sh.read_stats())
                 stats['shards'].append(one)
         else:
             stats = s.kernel_stats()
             stats.update(s.template_stats())
+            stats.update(s.read_stats())
         pts = []
         if 'metrics' in plan:
             # fan-out: points are tagged like the reference tags them

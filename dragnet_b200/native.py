@@ -92,6 +92,8 @@ _SIGS = [
      [_P, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_uint64),
       ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_double),
       ctypes.c_char_p, ctypes.c_size_t]),
+    ('dng_scan_read_stats', ctypes.c_int,
+     [_P] + [ctypes.POINTER(ctypes.c_uint64)] * 4),
     ('dng_scan_launch_count', ctypes.c_uint64, [_P]),
     ('dng_pinned_alloc', _P, [ctypes.c_size_t]),
     ('dng_pinned_free', None, [_P]),
@@ -167,6 +169,7 @@ def lib():
 
 
 JIT_CACHE_STATS = ['hits', 'misses', 'writes', 'evictions', 'errors']
+READ_STATS = ['direct_bytes', 'buffered_bytes', 'direct_ranges', 'fallbacks']
 
 
 def set_jit_cache_dir(path):
@@ -371,6 +374,18 @@ class _ScanStats(object):
                 'jit': {'state': int(st.value), 'launches': int(jl.value),
                         'compile_ms': cms.value, 'link_ms': lms.value,
                         'error': err.value.decode('utf-8', 'replace')}}
+
+
+    def read_stats(self):
+        """How dng_scan_feed_file read: bytes with O_DIRECT and through the
+        page cache, ranges read direct, ranges the filesystem refused
+        O_DIRECT for (read through the page cache).  A multi-device scan
+        gives its shards' sums."""
+        v = [ctypes.c_uint64() for _ in READ_STATS]
+        _check(lib().dng_scan_read_stats(self.handle,
+                                         *[ctypes.byref(x) for x in v]),
+               self.handle)
+        return dict(zip(READ_STATS, (int(x.value) for x in v)))
 
 
 class Scan(_ScanStats):

@@ -133,11 +133,13 @@ int dng_scan_open_devices(const dng_plan *plan, const int *devices, int n,
 /*
  * Shard i of a scan from dng_scan_open_devices (NULL for any other scan or
  * index), owned by that scan: for the stats calls only (kernel_kind,
- * kernel_stats, tally_stats, template_stats, jit_stats, launch_count, and
+ * kernel_stats, tally_stats, template_stats, jit_stats, launch_count,
+ * read_stats, and
  * counters after finish); never feed, finish or destroy it.  Shards learn
  * their templates from their own head and may pick different kernels;
  * results never depend on either.  Those stats calls on the multi-device scan
- * itself return DNG_EINVAL (dng_scan_launch_count sums the shards').
+ * itself return DNG_EINVAL (dng_scan_launch_count and dng_scan_read_stats
+ * sum the shards').
  */
 dng_scan *dng_scan_shard(const dng_scan *scan, int i);
 
@@ -159,7 +161,10 @@ int dng_scan_set_stream(dng_scan *scan, void *cuda_stream);
  *   buffer are only ENQUEUED when this returns (on the scan's stream, or the
  *   caller's after dng_scan_set_stream): like a pinned buffer, it must stay
  *   valid and unmodified until the next dng_scan_sync()/dng_scan_finish().
- * dng_scan_feed_file: read(2) the file into the pinned ring and feed it.
+ * dng_scan_feed_file: read the file into the pinned ring and feed it: with
+ *   O_DIRECT (storage straight into pinned memory, the page cache bypassed)
+ *   when little of it is in the page cache, else through the page cache
+ *   (dng_scan_read_stats).  Pipes and devices are read(2) in sequence.
  */
 int dng_scan_feed(dng_scan *scan, const void *buf, size_t len);
 int dng_scan_feed_pinned(dng_scan *scan, const void *buf, size_t len);
@@ -253,6 +258,15 @@ int dng_scan_kernel_kind(const dng_scan *scan);
  */
 int dng_scan_jit_stats(dng_scan *scan, int *state, uint64_t *launches,
     double *compile_ms, double *link_ms, char *err, size_t errlen);
+/* Bytes dng_scan_feed_file read with O_DIRECT (straight from storage into
+ * pinned memory) and through the page cache, and the files or shard ranges
+ * that were read direct.  Files mostly absent from the page cache are read
+ * direct; results never depend on it.  *fallbacks counts the ranges chosen
+ * for O_DIRECT that the filesystem refused (they are read through the page
+ * cache).  Regular files only; on a multi-device scan, the shards' sums.
+ * Any pointer may be NULL. */
+int dng_scan_read_stats(dng_scan *scan, uint64_t *direct_bytes,
+    uint64_t *buffered_bytes, uint64_t *direct_ranges, uint64_t *fallbacks);
 /* Every kernel this scan has launched so far: scan kernels plus the small
  * ones around them (template resolution, newline search of device feeds,
  * result compaction). */
