@@ -35,6 +35,7 @@
 #include "jit_cache.h"
 #include "gen.cuh"
 #include "direct_read.h"
+#include "inflate.cuh"
 
 using namespace dng;
 
@@ -174,6 +175,22 @@ struct dng_scan {
 	/* dng_scan_read_stats */
 	uint64_t direct_bytes = 0, buffered_bytes = 0, direct_ranges = 0;
 	uint64_t read_fallbacks = 0;
+	/* dng_scan_feed_gzip: files queued for the next inflate batch (path,
+	 * compressed size, output room), the batch's device buffers, stats */
+	struct GzFile {
+		std::string path;
+		size_t size;
+		uint64_t hint;
+	};
+	std::vector<GzFile> gz_queue;
+	uint64_t gz_queued_in = 0, gz_queued_out = 0;
+	u8 *d_gz_in = nullptr, *d_gz_out = nullptr, *d_gz_big = nullptr;
+	u8 *d_gz_join = nullptr;
+	size_t gz_in_cap = 0, gz_out_cap = 0, gz_big_cap = 0, gz_join_cap = 0;
+	u8 *d_gz_jobs = nullptr, *h_gz_jobs = nullptr;	/* jobs, results, next */
+	uint64_t gz_files = 0, gz_members = 0, gz_in_bytes = 0, gz_out_bytes = 0;
+	uint64_t gz_launches = 0;
+	double gz_ms = 0;
 	/* stats */
 	std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_pairs;
 	std::vector<cudaEvent_t> ev_pool;
@@ -1067,6 +1084,9 @@ int dng_scan_set_stream(dng_scan *s, void *cuda_stream)
 	return DNG_OK;
 }
 
+static int gz_flush(dng_scan *s);
+static int feed_device(dng_scan *s, const void *devbuf, size_t len);
+
 static int ensure_ring(dng_scan *s, bool need_stage)
 {
 	for (size_t i = 0; i < RING_SLOTS; i++) {
@@ -1091,7 +1111,7 @@ int dng_scan_feed(dng_scan *s, const void *buf, size_t len)
 	if (s->multi)
 		return refuse_multi(s, "dng_scan_feed");
 	cudaSetDevice(s->device);
-	if (ensure_ring(s, true))
+	if (gz_flush(s) || ensure_ring(s, true))
 		return s->err_code;
 	return feed_host(s, buf, len, false);
 }
@@ -1103,7 +1123,7 @@ int dng_scan_feed_pinned(dng_scan *s, const void *buf, size_t len)
 	if (s->multi)
 		return refuse_multi(s, "dng_scan_feed_pinned");
 	cudaSetDevice(s->device);
-	if (ensure_ring(s, false))
+	if (gz_flush(s) || ensure_ring(s, false))
 		return s->err_code;
 	return feed_host(s, buf, len, true);
 }
@@ -1172,7 +1192,7 @@ static int feed_fd_sequential(dng_scan *s, int fd, const char *path)
  * the threads.
  */
 static int feed_file_parallel(dng_scan *s, int fd, size_t off, size_t size,
-    const char *path, bool exact)
+    const char *path, bool exact, u8 *to_dev = nullptr)
 {
 	const size_t BLK = DR_BLK;
 	const size_t NSLOT = 32;	/* 128 MiB of pinned ring */
@@ -1277,9 +1297,16 @@ static int feed_file_parallel(dng_scan *s, int fd, size_t off, size_t size,
 		}
 		if (rc)
 			break;
-		if (bytes)
+		if (bytes && to_dev) {	/* (a gzip file: to its batch buffer) */
+			rc = s->cuda(cudaMemcpyAsync(to_dev, s->file_buf +
+			    (b % NSLOT) * BLK + r.plan.lo(b), bytes,
+			    cudaMemcpyHostToDevice, s->copy_stream),
+			    "cudaMemcpyAsync");
+			to_dev += bytes;
+		} else if (bytes) {
 			rc = feed_host(s, s->file_buf + (b % NSLOT) * BLK +
 			    r.plan.lo(b), bytes, true);
+		}
 		for (size_t j = 0; j < k && !rc; j++)
 			rc = s->cuda(cudaEventRecord(
 			    s->file_done[(b + j) % NSLOT], s->copy_stream),
@@ -1528,7 +1555,7 @@ int dng_scan_feed_file(dng_scan *s, const char *path)
 	if (s->multi)
 		return record_file(s, path);
 	cudaSetDevice(s->device);
-	if (ensure_ring(s, false))
+	if (gz_flush(s) || ensure_ring(s, false))
 		return s->err_code;
 	int fd = open(path, O_RDONLY);
 	if (fd < 0)
@@ -1550,6 +1577,15 @@ int dng_scan_feed_device(dng_scan *s, const void *devbuf, size_t len)
 		return DNG_EINVAL;
 	if (s->multi)
 		return refuse_multi(s, "dng_scan_feed_device");
+	cudaSetDevice(s->device);
+	if (gz_flush(s))
+		return s->err_code;
+	return feed_device(s, devbuf, len);
+}
+
+/* dng_scan_feed_device of a single-device scan with no gzip files queued */
+static int feed_device(dng_scan *s, const void *devbuf, size_t len)
+{
 	if (s->err_code)
 		return s->err_code;
 	if (s->finished)
@@ -1570,7 +1606,7 @@ int dng_scan_feed_device(dng_scan *s, const void *devbuf, size_t len)
 	const size_t LAUNCH_MAX = (size_t)4 << 30;
 	if (s->plan.dev.format == FMT_SKINNER && len > LAUNCH_MAX) {
 		for (size_t off = 0; off < len; off += LAUNCH_MAX) {
-			int rc = dng_scan_feed_device(s, (const u8 *)devbuf + off,
+			int rc = feed_device(s, (const u8 *)devbuf + off,
 			    std::min(LAUNCH_MAX, len - off));
 			if (rc)
 				return rc;
@@ -1669,6 +1705,285 @@ int dng_scan_feed_device(dng_scan *s, const void *devbuf, size_t len)
 	return 0;
 }
 
+/* ---- gzip files (dng_scan_feed_gzip) -------------------------------------
+ *
+ * Queued files are inflated in batches by inflate_kernel (inflate.cuh), one
+ * warp per file, into output regions laid out back to back in one device
+ * buffer, each as large as its file's ISIZE trailer says (exact for a single
+ * member under 4 GiB).  When every file filled its region exactly, the batch
+ * is fed as one device buffer (one newline search, one wait).  Otherwise
+ * each run of files that filled their regions is fed as one buffer, each file
+ * that did not on its own, and a file that ran out of room is decoded again,
+ * alone, in twice the room until it fits (several members, trailing zeros, or
+ * >= 4 GiB).
+ *
+ * A batch holds at most 2 GiB of output room, 512 MiB of compressed bytes
+ * and 256 files; a larger file goes alone.  One warp decodes one file, so a
+ * batch must hold several large files to decode them at once.  Its buffers
+ * (2.5 GiB) live beside the scan's own (table, arena, H2D ring: about
+ * 2.5 GiB at the defaults), far below an H100's 80 GB.  Every batch buffer is written on the
+ * scan's stream, after the scan kernels that read it earlier: a region stays
+ * valid until those kernels have finished, as dng_scan_feed_device needs.
+ */
+static const size_t GZ_BATCH_OUT = (size_t)2 << 30;
+static const size_t GZ_BATCH_IN = (size_t)512 << 20;
+static const size_t GZ_BATCH_FILES = 256;
+
+static size_t round16(size_t n)
+{
+	return (n + 15) & ~(size_t)15;
+}
+
+/* make *p hold at least n bytes (powers of two from 1 MiB, so the buffer
+ * cache takes them back); what the old buffer held is not kept */
+static int gz_room(dng_scan *s, u8 **p, size_t *cap, size_t n)
+{
+	if (*p && *cap >= n)
+		return 0;
+	size_t c = (size_t)1 << 20;
+	while (c < n)
+		c <<= 1;
+	if (*p) {
+		/* scan kernels enqueued earlier may still read it */
+		CK(s, cudaStreamSynchronize(s->stream));
+		cached_free(*p);
+		*p = nullptr;
+		*cap = 0;
+	}
+	CK(s, DEV_ALLOC(s, p, c));
+	*cap = c;
+	return 0;
+}
+
+/* one inflate launch over jobs[0, n) on the scan's stream, and its results:
+ * the one wait of a batch */
+static int gz_launch(dng_scan *s, const InfJob *jobs, u32 n, InfResult *out)
+{
+	const size_t jb = GZ_BATCH_FILES * sizeof (InfJob);
+	const size_t rb = GZ_BATCH_FILES * sizeof (InfResult);
+	if (!s->d_gz_jobs) {
+		CK(s, DEV_ALLOC(s, &s->d_gz_jobs, jb + rb + 64));
+		CK(s, HOST_ALLOC(&s->h_gz_jobs, jb + rb));
+	}
+	memcpy(s->h_gz_jobs, jobs, n * sizeof (InfJob));
+	CK(s, cudaMemcpyAsync(s->d_gz_jobs, s->h_gz_jobs, n * sizeof (InfJob),
+	    cudaMemcpyHostToDevice, s->stream));
+	u32 *d_next = (u32 *)(s->d_gz_jobs + jb + rb);
+	CK(s, cudaMemsetAsync(d_next, 0, sizeof (u32), s->stream));
+	cudaEvent_t e0 = get_event(s), e1 = get_event(s);
+	cudaEventRecord(e0, s->stream);
+	const u32 grid = std::min<u32>((n + INF_WARPS - 1) / INF_WARPS,
+	    (u32)s->sm_count * 4);
+	inflate_kernel<<<grid, 32 * INF_WARPS, 0, s->stream>>>(
+	    (const InfJob *)s->d_gz_jobs, (InfResult *)(s->d_gz_jobs + jb), n,
+	    d_next);
+	cudaError_t e = cudaGetLastError();
+	cudaEventRecord(e1, s->stream);
+	s->aux_launches++;
+	s->gz_launches++;
+	if (e == cudaSuccess)
+		e = cudaMemcpyAsync(s->h_gz_jobs + jb, s->d_gz_jobs + jb,
+		    n * sizeof (InfResult), cudaMemcpyDeviceToHost, s->stream);
+	if (e == cudaSuccess)
+		e = cudaStreamSynchronize(s->stream);
+	float ms = 0;
+	if (e == cudaSuccess && cudaEventElapsedTime(&ms, e0, e1) == cudaSuccess)
+		s->gz_ms += ms;
+	/* (back to the pool on every path: the stream is synchronized or
+	 * failed, and dng_scan_destroy waits for it before freeing them) */
+	s->ev_pool.push_back(e0);
+	s->ev_pool.push_back(e1);
+	if (s->cuda(e, "inflate_kernel"))
+		return s->err_code;
+	memcpy(out, s->h_gz_jobs + jb, n * sizeof (InfResult));
+	return 0;
+}
+
+static int gz_damage(dng_scan *s, const std::string &path, const InfResult &r)
+{
+	return s->fail(DNG_EIO, path + ": corrupt gzip data: " +
+	    inflate_error_name(r.kind) + " (compressed byte " +
+	    std::to_string(r.bit / 8) + ")");
+}
+
+/* inflate and feed the queued gzip files, in the order they were fed */
+static int gz_flush(dng_scan *s)
+{
+	if (s->gz_queue.empty())
+		return s->err_code;
+	std::vector<dng_scan::GzFile> q;
+	q.swap(s->gz_queue);
+	s->gz_queued_in = s->gz_queued_out = 0;
+	if (s->err_code)
+		return s->err_code;
+	const size_t n = q.size();
+	std::vector<size_t> in_off(n), out_off(n);
+	size_t tin = 0, tout = 0;
+	for (size_t i = 0; i < n; i++) {
+		in_off[i] = tin;
+		tin += round16(q[i].size);
+		out_off[i] = tout;
+		tout += q[i].hint;
+	}
+	if (gz_room(s, &s->d_gz_in, &s->gz_in_cap, tin) ||
+	    gz_room(s, &s->d_gz_out, &s->gz_out_cap, tout))
+		return s->err_code;
+	/* compressed bytes through the file reader (direct_read.h's policy) */
+	for (size_t i = 0; i < n; i++) {
+		const char *path = q[i].path.c_str();
+		int fd = open(path, O_RDONLY);
+		if (fd < 0)
+			return s->fail(DNG_EIO, std::string("open ") + path +
+			    ": " + strerror(errno));
+		const int rc = feed_file_parallel(s, fd, 0, q[i].size, path, true,
+		    s->d_gz_in + in_off[i]);
+		close(fd);
+		if (rc)
+			return rc;
+	}
+	/* largest first, so that no big file is left running alone */
+	std::vector<u32> order(n);
+	for (size_t i = 0; i < n; i++)
+		order[i] = (u32)i;
+	std::stable_sort(order.begin(), order.end(), [&](u32 a, u32 b) {
+		return q[a].size > q[b].size;
+	});
+	std::vector<InfJob> jobs(n);
+	for (size_t k = 0; k < n; k++) {
+		const u32 i = order[k];
+		jobs[k] = { s->d_gz_in + in_off[i], q[i].size,
+		    s->d_gz_out + out_off[i], q[i].hint };
+	}
+	std::vector<InfResult> res(n), by_file(n);
+	if (gz_launch(s, jobs.data(), (u32)n, res.data()))
+		return s->err_code;
+	for (size_t k = 0; k < n; k++)
+		by_file[order[k]] = res[k];
+	for (size_t i = 0; i < n; i++) {
+		if (by_file[i].status == INF_ERROR)
+			return gz_damage(s, q[i].path, by_file[i]);
+		s->gz_in_bytes += q[i].size;
+	}
+	s->gz_files += n;
+	/* in file order: each run of files that filled their regions exactly
+	 * is one feed (the whole batch when every hint held); a file that did
+	 * not is fed on its own, decoded again in more room if it ran out */
+	auto filled = [&](size_t i) {
+		return by_file[i].status == INF_DONE &&
+		    by_file[i].out_len == q[i].hint;
+	};
+	for (size_t i = 0, next; i < n; i = next) {
+		const u8 *src = s->d_gz_out + out_off[i];
+		uint64_t len = 0;
+		next = i + 1;
+		if (filled(i)) {
+			while (next < n && filled(next))
+				next++;
+			for (size_t k = i; k < next; k++) {
+				s->gz_members += by_file[k].members;
+				len += by_file[k].out_len;
+			}
+		} else {
+			InfResult r = by_file[i];
+			uint64_t cap = q[i].hint;
+			while (r.status == INF_ROOM) {
+				cap = std::max<uint64_t>(cap * 2,
+				    (uint64_t)1 << 20);
+				if (gz_room(s, &s->d_gz_big, &s->gz_big_cap, cap))
+					return s->err_code;
+				const InfJob j = { s->d_gz_in + in_off[i],
+				    q[i].size, s->d_gz_big, cap };
+				if (gz_launch(s, &j, 1, &r))
+					return s->err_code;
+				src = s->d_gz_big;
+			}
+			if (r.status == INF_ERROR)
+				return gz_damage(s, q[i].path, r);
+			s->gz_members += r.members;
+			len = r.out_len;
+		}
+		s->gz_out_bytes += len;
+		if (!len)
+			continue;	/* (an empty file adds nothing) */
+		if ((uintptr_t)src & 15) {
+			/* regions start where the hints before them end: a run
+			 * after a file that missed its hint is realigned */
+			if (gz_room(s, &s->d_gz_join, &s->gz_join_cap, len))
+				return s->err_code;
+			CK(s, cudaMemcpyAsync(s->d_gz_join, src, len,
+			    cudaMemcpyDeviceToDevice, s->stream));
+			src = s->d_gz_join;
+		}
+		if (feed_device(s, src, len))
+			return s->err_code;
+	}
+	return 0;
+}
+
+int dng_scan_feed_gzip(dng_scan *s, const char *path)
+{
+	if (!s || !path)
+		return DNG_EINVAL;
+	if (s->multi)
+		return refuse_multi(s, "dng_scan_feed_gzip");
+	if (s->err_code)
+		return s->err_code;
+	if (s->finished)
+		return s->fail(DNG_EINVAL, "scan already finished");
+	cudaSetDevice(s->device);
+	int fd = open(path, O_RDONLY);
+	if (fd < 0)
+		return s->fail(DNG_EIO, std::string("open ") + path + ": " +
+		    strerror(errno));
+	struct stat st;
+	u8 head[3] = {}, tail[4] = {};
+	const bool reg = fstat(fd, &st) == 0 && S_ISREG(st.st_mode);
+	const bool gz = reg && st.st_size >= 3 && pread(fd, head, 3, 0) == 3 &&
+	    head[0] == 0x1f && head[1] == 0x8b && head[2] == 8;
+	const bool trailer = gz && st.st_size >= 4 &&
+	    pread(fd, tail, 4, st.st_size - 4) == 4;
+	close(fd);
+	if (!gz) {
+		/* refused, not failed: the scan goes on */
+		if (!s->err_code)
+			s->err = std::string(path) + (reg ? ": not a gzip file "
+			    "(it does not start with 1f 8b 08)" :
+			    ": not a regular file");
+		return DNG_EINVAL;
+	}
+	const size_t size = (size_t)st.st_size;
+	const uint64_t hint = trailer ? inflate_hint(tail, size) : 0;
+	if (!s->gz_queue.empty() && (s->gz_queue.size() >= GZ_BATCH_FILES ||
+	    s->gz_queued_in + round16(size) > GZ_BATCH_IN ||
+	    s->gz_queued_out + hint > GZ_BATCH_OUT) && gz_flush(s))
+		return s->err_code;
+	s->gz_queue.push_back({ path, size, hint });
+	s->gz_queued_in += round16(size);
+	s->gz_queued_out += hint;
+	return DNG_OK;
+}
+
+int dng_scan_gzip_stats(dng_scan *s, uint64_t *files, uint64_t *members,
+    uint64_t *compressed_bytes, uint64_t *inflated_bytes, uint64_t *launches,
+    double *inflate_ms)
+{
+	if (!s)
+		return DNG_EINVAL;
+	if (files)
+		*files = s->gz_files;
+	if (members)
+		*members = s->gz_members;
+	if (compressed_bytes)
+		*compressed_bytes = s->gz_in_bytes;
+	if (inflated_bytes)
+		*inflated_bytes = s->gz_out_bytes;
+	if (launches)
+		*launches = s->gz_launches;
+	if (inflate_ms)
+		*inflate_ms = s->gz_ms;
+	return DNG_OK;
+}
+
 int dng_scan_sync(dng_scan *s)
 {
 	if (!s)
@@ -1676,6 +1991,7 @@ int dng_scan_sync(dng_scan *s)
 	if (s->multi)	/* (its shards run only inside dng_scan_finish) */
 		return s->err_code;
 	cudaSetDevice(s->device);
+	gz_flush(s);
 	CK(s, cudaStreamSynchronize(s->copy_stream));
 	CK(s, cudaStreamSynchronize(s->stream));
 	drain_events(s);
@@ -1788,7 +2104,7 @@ int dng_scan_finish(dng_scan *s, dng_result **out)
 	if (s->multi)
 		return finish_multi(s, out);
 	cudaSetDevice(s->device);
-	if (flush_tail(s))
+	if (gz_flush(s) || flush_tail(s))
 		return s->err_code;
 	if (dng_scan_sync(s))
 		return s->err_code;
@@ -2110,6 +2426,12 @@ void dng_scan_destroy(dng_scan *s)
 	cached_free(s->d_nl);
 	cached_free(s->d_carry);
 	cached_free(s->d_side);
+	cached_free(s->d_gz_in);
+	cached_free(s->d_gz_out);
+	cached_free(s->d_gz_big);
+	cached_free(s->d_gz_join);
+	cached_free(s->d_gz_jobs);
+	cached_free(s->h_gz_jobs);
 	if (s->own_stream)
 		cudaStreamDestroy(s->own_stream);
 	if (s->copy_stream)

@@ -93,15 +93,31 @@ def stage_counters(plan, c, npoints):
     return out
 
 
+GZIP_MAGIC = b'\x1f\x8b\x08'
+COMPRESSIONS = (None, 'none', 'gzip')
+
+
+def is_gzip(path):
+    """Whether the file starts as a gzip member of DEFLATE data does."""
+    with open(path, 'rb') as f:
+        return f.read(3) == GZIP_MAGIC
+
+
 def run_plan(plan, files=(), chunks=None, device=0, device_buffers=None,
-             templates=None, devices=None):
+             templates=None, devices=None, compression=None):
     """Drive one scan through the C ABI.  Input is any of: files (read by the
     library), host byte chunks, or (ptr, len) device buffers.  devices: more
     than one device index -> one scan over all of them, the files cut into a
-    byte range per device (files only); its stats are per shard."""
+    byte range per device (files only); its stats are per shard.
+    compression 'gzip': files that start with 1f 8b 08 are inflated on the
+    device (dng_scan_feed_gzip), others read as they are; one device only."""
     import json
-    p = native.Plan(json.dumps(plan, separators=(',', ':')))
     multi = devices is not None and len(devices) > 1
+    gzip = compression == 'gzip'
+    if gzip and multi:
+        raise DsError('compression "gzip" is not supported on a scan over '
+                      'several devices')
+    p = native.Plan(json.dumps(plan, separators=(',', ':')))
     if devices and not multi:
         device = devices[0]
     s = native.Scan(p, devices=list(devices)) if multi else \
@@ -110,7 +126,10 @@ def run_plan(plan, files=(), chunks=None, device=0, device_buffers=None,
         if templates is not None:
             s.set_templates(templates)
         for f in files:
-            s.feed_file(f)
+            if gzip and is_gzip(f):
+                s.feed_gzip(f)
+            else:
+                s.feed_file(f)
         for c in (chunks or ()):
             s.feed(c)
         for ptr, n in (device_buffers or ()):
@@ -128,6 +147,8 @@ def run_plan(plan, files=(), chunks=None, device=0, device_buffers=None,
             stats = s.kernel_stats()
             stats.update(s.template_stats())
             stats.update(s.read_stats())
+            if gzip:
+                stats.update(s.gzip_stats())
         pts = []
         if 'metrics' in plan:
             # fan-out: points are tagged like the reference tags them
@@ -171,6 +192,10 @@ class DatasourceGpu(object):
         # a list of device indices, or "all": one scan over all of them
         # (files cut by bytes, tallies merged exactly), else ds_device alone
         self.ds_devices = dsconfig.get('devices')
+        # "gzip": gzip files among the input are inflated on the device
+        self.ds_compression = bc.get('compression')
+        if self.ds_compression == 'none':
+            self.ds_compression = None
         # (root, timeFormat, after_ms, before_ms) -> [paths]: the reference's
         # own enumeration (lib/datasource-file.js:218-246 findStream), which
         # the real integration keeps; the tests pass their mirror of it
@@ -183,6 +208,14 @@ class DatasourceGpu(object):
         if self.ds_devices == 'all':
             return list(range(native.lib().dng_device_count()))
         return self.ds_devices
+
+    def _run(self, plan, files):
+        devices = self._devices()
+        if self.ds_compression == 'gzip' and devices and len(devices) > 1:
+            return DsError('compression "gzip" is not supported on a scan '
+                           'over several devices')
+        return run_plan(plan, files=files, device=self.ds_device,
+                        devices=devices, compression=self.ds_compression)
 
     def scan(self, args):
         """lib/datasource-file.js:72-108.  Returns ScanResult or an Error."""
@@ -204,8 +237,7 @@ class DatasourceGpu(object):
         plan = mod_query.scan_plan(query, ds_filter=self.ds_filter,
                                    time_field=self.ds_timefield,
                                    data_format=self.ds_format)
-        return run_plan(plan, files=files, device=self.ds_device,
-                        devices=self._devices())
+        return self._run(plan, files)
 
     def checkTimeArgs(self, args):
         """lib/datasource-file.js:549-556."""
@@ -237,8 +269,9 @@ class DatasourceGpu(object):
             plan = mod_query.scan_plan_multi(
                 queries[base:base + MAX_METRICS], ds_filter=self.ds_filter,
                 time_field=self.ds_timefield, data_format=self.ds_format)
-            r = run_plan(plan, files=files, device=self.ds_device,
-                         devices=self._devices())
+            r = self._run(plan, files)
+            if isinstance(r, DsError):
+                return r
             for fields, value in r.points:
                 fields[-1] = ('__dn_metric', base + fields[-1][1])
                 pts.append((fields, value))
@@ -294,6 +327,8 @@ class DatasourceGpu(object):
         t0 = time.perf_counter()
         res = self._fanout(args['metrics'], args['interval'], after, before,
                            files)
+        if isinstance(res, DsError):
+            return res
         t1 = time.perf_counter()
         written = mod_index.write_index(self.ds_indexpath, args['metrics'],
                                         args['interval'], res.points)
@@ -385,6 +420,9 @@ def createDatasource(args):
                     for d in devs)):
         return DsError('expected datasource "devices" to be "all" or a '
                        'non-empty list of device indices')
+    comp = bc.get('compression')
+    if comp not in COMPRESSIONS:
+        return DsError('unsupported compression: "%s"' % (comp,))
     return DatasourceGpu(args)
 
 

@@ -67,6 +67,7 @@ _SIGS = [
     ('dng_scan_feed_pinned', ctypes.c_int, [_P, _P, ctypes.c_size_t]),
     ('dng_scan_feed_device', ctypes.c_int, [_P, _P, ctypes.c_size_t]),
     ('dng_scan_feed_file', ctypes.c_int, [_P, ctypes.c_char_p]),
+    ('dng_scan_feed_gzip', ctypes.c_int, [_P, ctypes.c_char_p]),
     ('dng_scan_sync', ctypes.c_int, [_P]),
     ('dng_scan_finish', ctypes.c_int, [_P, ctypes.POINTER(_P)]),
     ('dng_scan_counters', ctypes.c_int, [_P, ctypes.POINTER(DngCounters)]),
@@ -94,6 +95,9 @@ _SIGS = [
       ctypes.c_char_p, ctypes.c_size_t]),
     ('dng_scan_read_stats', ctypes.c_int,
      [_P] + [ctypes.POINTER(ctypes.c_uint64)] * 4),
+    ('dng_scan_gzip_stats', ctypes.c_int,
+     [_P] + [ctypes.POINTER(ctypes.c_uint64)] * 5 +
+     [ctypes.POINTER(ctypes.c_double)]),
     ('dng_scan_launch_count', ctypes.c_uint64, [_P]),
     ('dng_pinned_alloc', _P, [ctypes.c_size_t]),
     ('dng_pinned_free', None, [_P]),
@@ -170,6 +174,8 @@ def lib():
 
 JIT_CACHE_STATS = ['hits', 'misses', 'writes', 'evictions', 'errors']
 READ_STATS = ['direct_bytes', 'buffered_bytes', 'direct_ranges', 'fallbacks']
+GZIP_STATS = ['gzip_files', 'gzip_members', 'gzip_compressed_bytes',
+              'gzip_inflated_bytes', 'inflate_launches', 'inflate_ms']
 
 
 def set_jit_cache_dir(path):
@@ -387,6 +393,17 @@ class _ScanStats(object):
                self.handle)
         return dict(zip(READ_STATS, (int(x.value) for x in v)))
 
+    def gzip_stats(self):
+        """What dng_scan_feed_gzip inflated: files, gzip members,
+        compressed and decompressed bytes, inflate kernel launches and
+        milliseconds."""
+        v = [ctypes.c_uint64() for _ in range(5)]
+        ms = ctypes.c_double()
+        _check(lib().dng_scan_gzip_stats(self.handle,
+                                         *[ctypes.byref(x) for x in v],
+                                         ctypes.byref(ms)), self.handle)
+        return dict(zip(GZIP_STATS, [int(x.value) for x in v] + [ms.value]))
+
 
 class Scan(_ScanStats):
     def __init__(self, plan, device=0, devices=None):
@@ -426,6 +443,12 @@ class Scan(_ScanStats):
 
     def feed_file(self, path):
         _check(lib().dng_scan_feed_file(self.handle, os.fsencode(path)),
+               self.handle)
+
+    def feed_gzip(self, path):
+        """A gzip file, inflated on the device; queued, and processed no
+        later than the next feed, sync or finish."""
+        _check(lib().dng_scan_feed_gzip(self.handle, os.fsencode(path)),
                self.handle)
 
     def sync(self):

@@ -172,6 +172,29 @@ int dng_scan_feed_device(dng_scan *scan, const void *devbuf, size_t len);
 int dng_scan_feed_file(dng_scan *scan, const char *path);
 int dng_scan_sync(dng_scan *scan);
 
+/*
+ * dng_scan_feed_gzip: a gzip file (RFC 1952: one or more members of DEFLATE
+ *   data, zero bytes after a member ignored, as Python's gzip.decompress
+ *   accepts), inflated on the device.  Its decompressed bytes join the scan's
+ *   stream at this point, exactly as dng_scan_feed_file of the decompressed
+ *   file would: `bytes` counts decompressed bytes, and a file without a
+ *   trailing newline joins its last line to the next file's first.  A file
+ *   that does not start with 1f 8b 08 fails here with DNG_EINVAL.  Files are
+ *   queued and inflated in batches, read as dng_scan_feed_file reads; the
+ *   queue is processed no later than the scan's next feed of any kind,
+ *   dng_scan_sync or dng_scan_finish, and a corrupt file (bad header, codes or
+ *   lengths, truncated, CRC-32 or ISIZE mismatch) fails the scan with DNG_EIO
+ *   from that call, naming the file and the damage.  A scan over several
+ *   devices refuses it (DNG_EINVAL).
+ */
+int dng_scan_feed_gzip(dng_scan *scan, const char *path);
+/* Gzip files inflated so far, their members, compressed and decompressed
+ * bytes, inflate kernel launches (one per batch, plus one per decode of a
+ * file again in more room) and their time (CUDA events). */
+int dng_scan_gzip_stats(dng_scan *scan, uint64_t *files, uint64_t *members,
+    uint64_t *compressed_bytes, uint64_t *inflated_bytes, uint64_t *launches,
+    double *inflate_ms);
+
 /* End of input: flushes the final unterminated line, then emits the points. */
 int dng_scan_finish(dng_scan *scan, dng_result **out);
 int dng_scan_counters(dng_scan *scan, dng_counters *out);

@@ -20,6 +20,7 @@
  */
 
 var mod_assertplus = require('assert-plus');
+var mod_fs = require('fs');
 var mod_stream = require('stream');
 var mod_vasync = require('vasync');
 var mod_vstream = require('vstream');
@@ -32,12 +33,25 @@ var jitCacheDirSet = false;
 
 exports.createDatasource = function createDatasource(args)
 {
-	var filecfg, fileds;
+	var filecfg, fileds, comp;
 
 	mod_assertplus.object(args.dsconfig);
 	mod_assertplus.optionalString(args.jitCacheDir, 'args.jitCacheDir');
 	if (typeof (args.dsconfig.ds_backend_config.path) != 'string')
 		return (new VError('expected datasource "path" to be a string'));
+	comp = args.dsconfig.ds_backend_config.compression;
+	if (comp !== undefined && comp !== 'none' && comp !== 'gzip')
+		return (new VError('unsupported compression: "%s"', comp));
+	/*
+	 * "all" on a host with one GPU is a scan on that GPU and reads gzip
+	 * files, as in DatasourceGpu in Python; on several GPUs the scan over
+	 * all of them refuses feedGzip with DNG_EINVAL.
+	 */
+	if (comp === 'gzip' &&
+	    Array.isArray(args.dsconfig.ds_backend_config.devices) &&
+	    args.dsconfig.ds_backend_config.devices.length > 1)
+		return (new VError('compression "gzip" is not supported on a ' +
+		    'scan over several devices'));
 
 	/* (before the first scan is opened) */
 	if (args.jitCacheDir !== undefined && !jitCacheDirSet) {
@@ -69,8 +83,45 @@ function DatasourceGpu(args, fileds)
 	 */
 	if (args.dsconfig.ds_backend_config.devices !== undefined)
 		this.ds_device = args.dsconfig.ds_backend_config.devices;
+	/*
+	 * "compression": "gzip": files that start with 1f 8b 08 (rotated logs)
+	 * are inflated on the GPU (dng_scan_feed_gzip), any other file (the
+	 * live log beside them) is read as it is.
+	 */
+	this.ds_gzip = args.dsconfig.ds_backend_config.compression === 'gzip';
 	this.ds_log = args.log;
 }
+
+/*
+ * Feed one file to a scan: feedGzip() for a gzip file when the datasource
+ * reads them, else feedFile().  Both are N-API async work items.
+ */
+DatasourceGpu.prototype.feedPath = function (scan, path, callback)
+{
+	if (!this.ds_gzip) {
+		scan.feedFile(path, callback);
+		return;
+	}
+	mod_fs.open(path, 'r', function (err, fd) {
+		if (err) {
+			callback(err);
+			return;
+		}
+		var head = Buffer.alloc(3);
+		mod_fs.read(fd, head, 0, 3, 0, function (rerr, n) {
+			mod_fs.close(fd, function () {});
+			if (rerr) {
+				callback(rerr);
+				return;
+			}
+			if (n == 3 && head[0] == 0x1f && head[1] == 0x8b &&
+			    head[2] == 0x08)
+				scan.feedGzip(path, callback);
+			else
+				scan.feedFile(path, callback);
+		});
+	});
+};
 
 /* metrics one fan-out plan may hold (MAX_METRICS, csrc/plan.h) */
 var MAX_METRICS = 8;
@@ -122,7 +173,7 @@ DatasourceGpu.prototype.scan = function (args)
 		if (fileinfo.error)
 			return;
 		scanctx.findstream.pause();
-		scan.feedFile(fileinfo.path, function (err) {
+		self.feedPath(scan, fileinfo.path, function (err) {
 			if (err)
 				out.emit('error', err);
 			else
@@ -310,6 +361,7 @@ DatasourceGpu.prototype.indexScanImpl = function (args, callback)
 DatasourceGpu.prototype.fanoutPass = function (queries, base, dsfilter, paths,
     sink, callback)
 {
+	var self = this;
 	var names, plan, scan;
 
 	names = [];
@@ -332,7 +384,9 @@ DatasourceGpu.prototype.fanoutPass = function (queries, base, dsfilter, paths,
 	}
 	mod_vasync.forEachPipeline({
 	    'inputs': paths,
-	    'func': function (path, feedcb) { scan.feedFile(path, feedcb); }
+	    'func': function (path, feedcb) {
+		self.feedPath(scan, path, feedcb);
+	    }
 	}, function (err) {
 		if (err) {
 			scan.close();
