@@ -36,6 +36,8 @@
 #include "gen.cuh"
 #include "direct_read.h"
 #include "inflate.cuh"
+#include "inflate_policy.h"
+#include "inflate_split.cuh"
 
 using namespace dng;
 
@@ -191,6 +193,15 @@ struct dng_scan {
 	uint64_t gz_files = 0, gz_members = 0, gz_in_bytes = 0, gz_out_bytes = 0;
 	uint64_t gz_launches = 0;
 	double gz_ms = 0;
+	/* the split path (inflate_split.cuh): a batch's chunk state, symbols,
+	 * outputs that missed their regions and checks; its stats */
+	u8 *d_gz_split = nullptr, *d_gz_sym = nullptr, *d_gz_sout = nullptr;
+	u8 *d_gz_check = nullptr;
+	size_t gz_split_cap = 0, gz_sym_cap = 0, gz_sout_cap = 0;
+	size_t gz_check_cap = 0;
+	uint64_t gz_split_files = 0, gz_chunks = 0, gz_false_starts = 0;
+	uint64_t gz_fallbacks = 0, gz_split_launches = 0;
+	uint32_t gz_split_blocks = 0;	/* CTAs of split_decode_kernel per SM */
 	/* stats */
 	std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_pairs;
 	std::vector<cudaEvent_t> ev_pool;
@@ -1718,8 +1729,8 @@ static int feed_device(dng_scan *s, const void *devbuf, size_t len)
  * >= 4 GiB).
  *
  * A batch holds at most 2 GiB of output room, 512 MiB of compressed bytes
- * and 256 files; a larger file goes alone.  One warp decodes one file, so a
- * batch must hold several large files to decode them at once.  Its buffers
+ * and 256 files; a larger file goes alone.  One warp decodes one file, except
+ * the large files of a batch of few, which are split (below).  Its buffers
  * (2.5 GiB) live beside the scan's own (table, arena, H2D ring: about
  * 2.5 GiB at the defaults), far below an H100's 80 GB.  Every batch buffer is written on the
  * scan's stream, after the scan kernels that read it earlier: a region stays
@@ -1806,6 +1817,407 @@ static int gz_damage(dng_scan *s, const std::string &path, const InfResult &r)
 	    std::to_string(r.bit / 8) + ")");
 }
 
+/* ---- gzip files split into chunks (inflate_split.cuh) ----------------------
+ *
+ * A batch with fewer files than the device holds decode warps cuts its large
+ * files into chunks (gz_split_plan, inflate_policy.h).  Before the batch's
+ * one wait: split_find_kernel finds each chunk's candidate block start and
+ * split_decode_kernel decodes every chunk into 16-bit symbols.  After it the
+ * host chains each file's chunks; a chain that ends in a chunk out of room
+ * decodes that chunk, and each later one that ran out, again in four times
+ * the room and member slots.  Then split_tail_kernel and split_body_kernel
+ * write each file's bytes, into its region when its length is the hint and
+ * into d_gz_sout otherwise, and split_crc_kernel and split_member_kernel
+ * check every member.  A file the split path cannot vouch for is decoded
+ * again by inflate_kernel, whose answer stands.
+ *
+ * Scratch, from the buffer cache: 16-bit symbols for 1.25 times each split
+ * file's hint plus 32 Ki symbols per chunk (2.5 times the batch's output
+ * room, plus 64 KiB per chunk), and four times that for each chunk decoded
+ * again; per chunk its candidate, job, result and four member slots; the
+ * pieces and members of the checks.
+ */
+struct GzChunk {		/* host state of one chunk */
+	SplitJob job;
+	SplitRes res;
+	std::vector<InfMember> mem;
+};
+
+struct GzSplitFile {
+	size_t file;			/* in the batch */
+	uint32_t first, n;		/* its chunks in the batch's list */
+	int chain;
+	std::vector<uint32_t> proven;
+	SplitLayout lay;
+	u8 *dst;
+	bool ok;
+};
+
+static uint64_t gz_resident(dng_scan *s)
+{
+	if (!s->gz_split_blocks) {
+		int b = 0;
+		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b,
+		    split_decode_kernel, 32 * SPLIT_WARPS, 0);
+		s->gz_split_blocks = b > 0 ? (uint32_t)b : 1;
+	}
+	return (uint64_t)s->gz_split_blocks * SPLIT_WARPS * s->sm_count;
+}
+
+/* time a stretch of split kernels into inflate_ms, once the stream is idle */
+struct GzTimer {
+	cudaEvent_t e0, e1;
+};
+
+static GzTimer gz_timer_start(dng_scan *s)
+{
+	GzTimer t = { get_event(s), get_event(s) };
+	cudaEventRecord(t.e0, s->stream);
+	return t;
+}
+
+static void gz_timer_stop(dng_scan *s, GzTimer &t)
+{
+	cudaEventRecord(t.e1, s->stream);
+}
+
+static void gz_timer_read(dng_scan *s, GzTimer &t)
+{
+	float ms = 0;
+	if (cudaEventElapsedTime(&ms, t.e0, t.e1) == cudaSuccess)
+		s->gz_ms += ms;
+	s->ev_pool.push_back(t.e0);
+	s->ev_pool.push_back(t.e1);
+}
+
+static void gz_split_count(dng_scan *s, uint32_t launches)
+{
+	s->gz_split_launches += launches;
+	s->aux_launches += launches;
+}
+
+/* split_decode_kernel over the chunks `which` (their jobs set), on the
+ * stream; device records at d_jobs / d_res */
+static int gz_split_decode(dng_scan *s, std::vector<GzChunk> &ck,
+    const std::vector<uint32_t> &which, u8 *d_jobs, u8 *d_res, u32 *d_next)
+{
+	const size_t n = which.size();
+	std::vector<SplitJob> jobs(n);
+	for (size_t i = 0; i < n; i++)
+		jobs[i] = ck[which[i]].job;
+	CK(s, cudaMemcpyAsync(d_jobs, jobs.data(), n * sizeof (SplitJob),
+	    cudaMemcpyHostToDevice, s->stream));
+	CK(s, cudaMemsetAsync(d_next, 0, sizeof (u32), s->stream));
+	gz_resident(s);
+	const u32 grid = std::min<u32>((u32)((n + SPLIT_WARPS - 1) / SPLIT_WARPS),
+	    s->gz_split_blocks * (u32)s->sm_count);
+	split_decode_kernel<<<grid, 32 * SPLIT_WARPS, 0, s->stream>>>(
+	    (const SplitJob *)d_jobs, (SplitRes *)d_res, (u32)n, d_next);
+	gz_split_count(s, 1);
+	CK(s, cudaGetLastError());
+	return 0;
+}
+
+/* 1 and 2: enqueue the finder and the first decode of every chunk of the
+ * split files (no wait) */
+static int gz_split_start(dng_scan *s, const std::vector<dng_scan::GzFile> &q,
+    const std::vector<size_t> &in_off, const std::vector<u32> &nch,
+    std::vector<GzSplitFile> &sf, std::vector<GzChunk> &ck, GzTimer &t)
+{
+	uint32_t total = 0;
+	uint64_t room = 0;
+	for (size_t i = 0; i < q.size(); i++) {
+		if (nch[i] < 2)
+			continue;
+		GzSplitFile f = {};
+		f.file = i;
+		f.first = total;
+		f.n = nch[i];
+		sf.push_back(f);
+		total += nch[i];
+	}
+	ck.resize(total);
+	for (const GzSplitFile &f : sf) {
+		const dng_scan::GzFile &g = q[f.file];
+		for (uint32_t k = 0; k < f.n; k++) {
+			const uint64_t cb = split_cut(g.size, f.n, k + 1) -
+			    split_cut(g.size, f.n, k);
+			SplitJob &j = ck[f.first + k].job;
+			j = {};
+			j.in = s->d_gz_in + in_off[f.file];
+			j.in_len = g.size;
+			j.cap = split_room(g.hint, g.size, cb);
+			j.k = k;
+			j.nchunks = f.n;
+			j.mcap = SPLIT_MSLOTS;
+			room += j.cap;
+		}
+	}
+	/* candidates | find jobs | decode jobs | results | member slots | next */
+	const size_t oc = 0, of = oc + total * sizeof (uint64_t),
+	    oj = of + total * sizeof (SplitFind),
+	    orr = oj + total * sizeof (SplitJob),
+	    om = orr + total * sizeof (SplitRes),
+	    on = om + (size_t)total * SPLIT_MSLOTS * sizeof (InfMember);
+	if (gz_room(s, &s->d_gz_split, &s->gz_split_cap, on + 16) ||
+	    gz_room(s, &s->d_gz_sym, &s->gz_sym_cap, room * 2))
+		return s->err_code;
+	uint64_t *d_cand = (uint64_t *)(s->d_gz_split + oc);
+	std::vector<SplitFind> finds;
+	uint64_t sym = 0;
+	for (const GzSplitFile &f : sf) {
+		const dng_scan::GzFile &g = q[f.file];
+		for (uint32_t k = 0; k < f.n; k++) {
+			SplitJob &j = ck[f.first + k].job;
+			j.cand = d_cand + f.first;
+			j.out = (uint16_t *)s->d_gz_sym + sym;
+			j.mem = (InfMember *)(s->d_gz_split + om) +
+			    (size_t)(f.first + k) * SPLIT_MSLOTS;
+			sym += j.cap;
+			if (k)
+				finds.push_back({ j.in, g.size,
+				    split_cut(g.size, f.n, k) * 8,
+				    split_cut(g.size, f.n, k + 1) * 8,
+				    d_cand + f.first + k });
+		}
+	}
+	CK(s, cudaMemcpyAsync(s->d_gz_split + of, finds.data(),
+	    finds.size() * sizeof (SplitFind), cudaMemcpyHostToDevice,
+	    s->stream));
+	t = gz_timer_start(s);
+	const u32 grid = std::min<u32>((u32)finds.size(), (u32)s->sm_count * 6);
+	split_find_kernel<<<grid, 32, 0, s->stream>>>(
+	    (const SplitFind *)(s->d_gz_split + of), (u32)finds.size());
+	gz_split_count(s, 1);
+	CK(s, cudaGetLastError());
+	std::vector<uint32_t> all(total);
+	for (uint32_t c = 0; c < total; c++)
+		all[c] = c;
+	if (gz_split_decode(s, ck, all, s->d_gz_split + oj,
+	    s->d_gz_split + orr, (u32 *)(s->d_gz_split + on)))
+		return s->err_code;
+	gz_timer_stop(s, t);
+	return 0;
+}
+
+/* results of chunks `which`, decoded into d_res, and their member records
+ * from the slots [d_mem, + nslots) their jobs point into */
+static int gz_split_collect(dng_scan *s, std::vector<GzChunk> &ck,
+    const std::vector<uint32_t> &which, const u8 *d_res,
+    const InfMember *d_mem, size_t nslots)
+{
+	std::vector<SplitRes> r(which.size());
+	std::vector<InfMember> m(nslots);
+	CK(s, cudaMemcpyAsync(r.data(), d_res, r.size() * sizeof (SplitRes),
+	    cudaMemcpyDeviceToHost, s->stream));
+	CK(s, cudaMemcpyAsync(m.data(), d_mem, nslots * sizeof (InfMember),
+	    cudaMemcpyDeviceToHost, s->stream));
+	CK(s, cudaStreamSynchronize(s->stream));
+	for (size_t i = 0; i < which.size(); i++) {
+		GzChunk &c = ck[which[i]];
+		c.res = r[i];
+		const InfMember *h = m.data() + (c.job.mem - d_mem);
+		c.mem.assign(h, h + c.res.members);
+	}
+	return 0;
+}
+
+/*
+ * 3 to 5, after the batch's wait: chain, decode again what ran out of room,
+ * resolve and check.  by_file[i] of a split file: DONE with its length and
+ * members (alt[i]: where its bytes are when not in its region), or ROOM,
+ * to be decoded whole (a fallback).
+ */
+static int gz_split_finish(dng_scan *s, const std::vector<dng_scan::GzFile> &q,
+    const std::vector<size_t> &out_off, std::vector<GzSplitFile> &sf,
+    std::vector<GzChunk> &ck, std::vector<InfResult> &by_file,
+    std::vector<const u8 *> &alt)
+{
+	std::vector<uint32_t> all(ck.size());
+	for (uint32_t c = 0; c < ck.size(); c++)
+		all[c] = c;
+	const size_t orr = ck.size() * (sizeof (uint64_t) + sizeof (SplitFind) +
+	    sizeof (SplitJob)), om = orr + ck.size() * sizeof (SplitRes);
+	if (gz_split_collect(s, ck, all, s->d_gz_split + orr,
+	    (const InfMember *)(s->d_gz_split + om), ck.size() * SPLIT_MSLOTS))
+		return s->err_code;
+	std::vector<u8 *> extra;	/* rooms of chunks decoded again */
+	struct Free {
+		std::vector<u8 *> &v;
+		~Free() { for (u8 *p : v) cached_free(p); }
+	} free_extra = { extra };
+	for (;;) {
+		std::vector<uint32_t> redo, r;
+		for (GzSplitFile &f : sf) {
+			std::vector<SplitRes> res(f.n);
+			for (uint32_t k = 0; k < f.n; k++)
+				res[k] = ck[f.first + k].res;
+			f.chain = split_chain(res.data(), f.proven);
+			if (f.chain != CHAIN_ROOM)
+				continue;
+			split_redo(res.data(), f.n, f.proven, r);
+			for (const uint32_t k : r)
+				redo.push_back(f.first + k);
+		}
+		if (redo.empty())
+			break;
+		uint64_t room = 0, slots = 0;
+		for (const uint32_t c : redo) {
+			room += ck[c].job.cap * 4;
+			slots += ck[c].job.mcap * 4;
+		}
+		const size_t bj = redo.size() * sizeof (SplitJob),
+		    br = redo.size() * sizeof (SplitRes),
+		    bm = slots * sizeof (InfMember);
+		u8 *d = nullptr;
+		CK(s, DEV_ALLOC(s, &d, room * 2 + bj + br + bm + 16));
+		extra.push_back(d);
+		uint64_t sym = 0, slot = 0;
+		for (const uint32_t c : redo) {
+			SplitJob &j = ck[c].job;
+			j.cap *= 4;
+			j.mcap *= 4;
+			j.out = (uint16_t *)d + sym;
+			j.mem = (InfMember *)(d + room * 2 + bj + br) + slot;
+			sym += j.cap;
+			slot += j.mcap;
+		}
+		GzTimer t = gz_timer_start(s);
+		if (gz_split_decode(s, ck, redo, d + room * 2, d + room * 2 + bj,
+		    (u32 *)(d + room * 2 + bj + br + bm)))
+			return s->err_code;
+		gz_timer_stop(s, t);
+		const int rc = gz_split_collect(s, ck, redo, d + room * 2 + bj,
+		    (const InfMember *)(d + room * 2 + bj + br), slots);
+		gz_timer_read(s, t);
+		if (rc)
+			return rc;
+	}
+	/* lay out every file whose chain reached the end */
+	size_t sout = 0;
+	for (GzSplitFile &f : sf) {
+		f.ok = f.chain == CHAIN_END;
+		s->gz_split_files++;
+		s->gz_chunks += f.n;
+		if (!f.ok)
+			continue;
+		std::vector<SplitRes> res(f.n);
+		std::vector<const InfMember *> mem(f.n);
+		for (uint32_t k = 0; k < f.n; k++) {
+			res[k] = ck[f.first + k].res;
+			mem[k] = ck[f.first + k].mem.data();
+		}
+		s->gz_false_starts += split_false_starts(res.data(), f.n,
+		    f.proven);
+		split_layout(res.data(), mem.data(), f.proven, f.lay);
+		if (f.lay.len != q[f.file].hint)
+			sout += round16(f.lay.len);
+	}
+	if (sout && gz_room(s, &s->d_gz_sout, &s->gz_sout_cap, sout))
+		return s->err_code;
+	/* resolve pieces | first | bad | CRC pieces | CRCs | members */
+	std::vector<SplitPiece> pieces;
+	std::vector<u32> first;
+	std::vector<CrcPiece> cp;
+	std::vector<CrcMember> cm;
+	std::vector<GzSplitFile *> okf;
+	sout = 0;
+	for (GzSplitFile &f : sf) {
+		if (!f.ok)
+			continue;
+		const u32 fi = (u32)okf.size();
+		okf.push_back(&f);
+		if (f.lay.len == q[f.file].hint) {
+			f.dst = s->d_gz_out + out_off[f.file];
+		} else {
+			f.dst = s->d_gz_sout + sout;
+			sout += round16(f.lay.len);
+		}
+		first.push_back((u32)pieces.size());
+		for (size_t i = 0; i < f.proven.size(); i++) {
+			const GzChunk &c = ck[f.first + f.proven[i]];
+			pieces.push_back({ c.job.out, f.dst, f.lay.off[i],
+			    c.res.out_len, f.lay.minidx[i], fi });
+		}
+		for (size_t m = 0; m < f.lay.mstart.size(); m++) {
+			CrcMember x = { (u32)cp.size(), 0, f.lay.crc[m],
+			    f.lay.isize[m], f.lay.mend[m] - f.lay.mstart[m], fi,
+			    0 };
+			for (uint64_t a = f.lay.mstart[m]; a < f.lay.mend[m];
+			    a += SPLIT_CRC_PIECE)
+				cp.push_back({ f.dst + a, std::min<uint64_t>(
+				    SPLIT_CRC_PIECE, f.lay.mend[m] - a) });
+			x.p1 = (u32)cp.size();
+			cm.push_back(x);
+		}
+	}
+	first.push_back((u32)pieces.size());
+	const size_t nok = okf.size();
+	std::vector<u32> bad(nok, 0);
+	if (nok) {
+		const size_t o1 = pieces.size() * sizeof (SplitPiece),
+		    o2 = o1 + first.size() * sizeof (u32),
+		    o3 = (o2 + nok * sizeof (u32) + 15) & ~(size_t)15,
+		    o4 = o3 + cp.size() * sizeof (CrcPiece),
+		    o5 = (o4 + cp.size() * sizeof (u32) + 15) & ~(size_t)15,
+		    o6 = o5 + cm.size() * sizeof (CrcMember);
+		if (gz_room(s, &s->d_gz_check, &s->gz_check_cap, o6))
+			return s->err_code;
+		u8 *d = s->d_gz_check;
+		CK(s, cudaMemcpyAsync(d, pieces.data(), o1,
+		    cudaMemcpyHostToDevice, s->stream));
+		CK(s, cudaMemcpyAsync(d + o1, first.data(), o2 - o1,
+		    cudaMemcpyHostToDevice, s->stream));
+		CK(s, cudaMemsetAsync(d + o2, 0, nok * sizeof (u32), s->stream));
+		if (!cp.empty())
+			CK(s, cudaMemcpyAsync(d + o3, cp.data(), o4 - o3,
+			    cudaMemcpyHostToDevice, s->stream));
+		if (!cm.empty())
+			CK(s, cudaMemcpyAsync(d + o5, cm.data(), o6 - o5,
+			    cudaMemcpyHostToDevice, s->stream));
+		u32 *d_bad = (u32 *)(d + o2);
+		GzTimer t = gz_timer_start(s);
+		split_tail_kernel<<<(u32)nok, 1024, 0, s->stream>>>(
+		    (const SplitPiece *)d, (const u32 *)(d + o1), d_bad);
+		split_body_kernel<<<(u32)pieces.size(), 256, 0, s->stream>>>(
+		    (const SplitPiece *)d, d_bad);
+		gz_split_count(s, 2);
+		if (!cp.empty()) {
+			split_crc_kernel<<<(u32)((cp.size() + 255) / 256), 256, 0,
+			    s->stream>>>((const CrcPiece *)(d + o3),
+			    (u32 *)(d + o4), (u32)cp.size());
+			split_member_kernel<<<(u32)((cm.size() + 3) / 4), 128, 0,
+			    s->stream>>>((const CrcMember *)(d + o5),
+			    (u32)cm.size(), (const CrcPiece *)(d + o3),
+			    (const u32 *)(d + o4), d_bad);
+			gz_split_count(s, 2);
+		}
+		gz_timer_stop(s, t);
+		CK(s, cudaGetLastError());
+		CK(s, cudaMemcpyAsync(bad.data(), d_bad, nok * sizeof (u32),
+		    cudaMemcpyDeviceToHost, s->stream));
+		CK(s, cudaStreamSynchronize(s->stream));
+		gz_timer_read(s, t);
+	}
+	for (size_t fi = 0; fi < nok; fi++)
+		okf[fi]->ok = !bad[fi];
+	for (const GzSplitFile &f : sf) {
+		InfResult &r = by_file[f.file];
+		r = {};
+		if (!f.ok) {
+			r.status = INF_ROOM;	/* decoded whole */
+			s->gz_fallbacks++;
+			continue;
+		}
+		r.status = INF_DONE;
+		r.out_len = f.lay.len;
+		r.members = (uint32_t)f.lay.mstart.size();
+		if (f.dst != s->d_gz_out + out_off[f.file])
+			alt[f.file] = f.dst;
+	}
+	return 0;
+}
+
 /* inflate and feed the queued gzip files, in the order they were fed */
 static int gz_flush(dng_scan *s)
 {
@@ -1841,24 +2253,64 @@ static int gz_flush(dng_scan *s)
 		if (rc)
 			return rc;
 	}
-	/* largest first, so that no big file is left running alone */
-	std::vector<u32> order(n);
+	/* large files of a batch of few: split (inflate_policy.h) */
+	std::vector<uint64_t> sizes(n);
 	for (size_t i = 0; i < n; i++)
-		order[i] = (u32)i;
+		sizes[i] = q[i].size;
+	std::vector<u32> nch(n);
+	gz_split_plan(sizes.data(), n, gz_resident(s), DNG_GZ_SPLIT_FLOOR,
+	    nch.data());
+	std::vector<GzSplitFile> sf;
+	std::vector<GzChunk> ck;
+	GzTimer st = {};
+	for (size_t i = 0; i < n; i++)
+		if (nch[i] > 1) {
+			if (gz_split_start(s, q, in_off, nch, sf, ck, st))
+				return s->err_code;
+			break;
+		}
+	/* the rest one warp each, largest first, so that no big file is left
+	 * running alone */
+	std::vector<u32> order;
+	for (size_t i = 0; i < n; i++)
+		if (nch[i] < 2)
+			order.push_back((u32)i);
 	std::stable_sort(order.begin(), order.end(), [&](u32 a, u32 b) {
 		return q[a].size > q[b].size;
 	});
-	std::vector<InfJob> jobs(n);
-	for (size_t k = 0; k < n; k++) {
-		const u32 i = order[k];
-		jobs[k] = { s->d_gz_in + in_off[i], q[i].size,
-		    s->d_gz_out + out_off[i], q[i].hint };
-	}
-	std::vector<InfResult> res(n), by_file(n);
-	if (gz_launch(s, jobs.data(), (u32)n, res.data()))
+	auto whole = [&](const std::vector<u32> &files,
+	    std::vector<InfResult> &by) {
+		std::vector<InfJob> jobs(files.size());
+		std::vector<InfResult> res(files.size());
+		for (size_t k = 0; k < files.size(); k++) {
+			const u32 i = files[k];
+			jobs[k] = { s->d_gz_in + in_off[i], q[i].size,
+			    s->d_gz_out + out_off[i], q[i].hint };
+		}
+		if (gz_launch(s, jobs.data(), (u32)files.size(), res.data()))
+			return s->err_code;
+		for (size_t k = 0; k < files.size(); k++)
+			by[files[k]] = res[k];
+		return 0;
+	};
+	std::vector<InfResult> by_file(n);
+	std::vector<const u8 *> alt(n, nullptr);
+	if (!order.empty() && whole(order, by_file))
 		return s->err_code;
-	for (size_t k = 0; k < n; k++)
-		by_file[order[k]] = res[k];
+	if (!sf.empty()) {
+		if (order.empty())
+			CK(s, cudaStreamSynchronize(s->stream));
+		gz_timer_read(s, st);
+		if (gz_split_finish(s, q, out_off, sf, ck, by_file, alt))
+			return s->err_code;
+		/* what the split path could not vouch for, decoded whole */
+		std::vector<u32> again;
+		for (const GzSplitFile &f : sf)
+			if (!f.ok)
+				again.push_back((u32)f.file);
+		if (!again.empty() && whole(again, by_file))
+			return s->err_code;
+	}
 	for (size_t i = 0; i < n; i++) {
 		if (by_file[i].status == INF_ERROR)
 			return gz_damage(s, q[i].path, by_file[i]);
@@ -1885,6 +2337,8 @@ static int gz_flush(dng_scan *s)
 			}
 		} else {
 			InfResult r = by_file[i];
+			if (alt[i])	/* split, and not the hint's length */
+				src = alt[i];
 			uint64_t cap = q[i].hint;
 			while (r.status == INF_ROOM) {
 				cap = std::max<uint64_t>(cap * 2,
@@ -1981,6 +2435,25 @@ int dng_scan_gzip_stats(dng_scan *s, uint64_t *files, uint64_t *members,
 		*launches = s->gz_launches;
 	if (inflate_ms)
 		*inflate_ms = s->gz_ms;
+	return DNG_OK;
+}
+
+int dng_scan_gzip_split_stats(dng_scan *s, uint64_t *split_files,
+    uint64_t *chunks, uint64_t *false_starts, uint64_t *fallbacks,
+    uint64_t *launches)
+{
+	if (!s)
+		return DNG_EINVAL;
+	if (split_files)
+		*split_files = s->gz_split_files;
+	if (chunks)
+		*chunks = s->gz_chunks;
+	if (false_starts)
+		*false_starts = s->gz_false_starts;
+	if (fallbacks)
+		*fallbacks = s->gz_fallbacks;
+	if (launches)
+		*launches = s->gz_split_launches;
 	return DNG_OK;
 }
 
@@ -2432,6 +2905,10 @@ void dng_scan_destroy(dng_scan *s)
 	cached_free(s->d_gz_join);
 	cached_free(s->d_gz_jobs);
 	cached_free(s->h_gz_jobs);
+	cached_free(s->d_gz_split);
+	cached_free(s->d_gz_sym);
+	cached_free(s->d_gz_sout);
+	cached_free(s->d_gz_check);
 	if (s->own_stream)
 		cudaStreamDestroy(s->own_stream);
 	if (s->copy_stream)

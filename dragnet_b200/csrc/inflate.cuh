@@ -96,6 +96,7 @@ inline uint64_t inflate_hint(const uint8_t *tail, uint64_t in_len)
 /* decode tables of one block, in the warp's shared memory; an entry of a fast
  * table is (symbol << 4) | length, 0 for "not a code of <= its bits" */
 struct InfTables {
+	enum { LBITS = INF_LBITS, DBITS = INF_DBITS };
 	uint16_t lcount[16], loffs[16], lfirst[16];
 	uint16_t dcount[16], doffs[16], dfirst[16];
 	uint16_t lsym[288], dsym[32];
@@ -115,13 +116,37 @@ struct InfLanes {
 	{
 		return __shfl_sync(0xffffffffu, v, src);
 	}
+	__device__ uint32_t ballot(bool v) const
+	{
+		return __ballot_sync(0xffffffffu, v);
+	}
 #else
 	uint32_t lane() const { return 0; }
 	uint32_t n() const { return 1; }
 	void sync() const {}
 	uint32_t bcast(uint32_t v, uint32_t) const { return v; }
+	uint32_t ballot(bool v) const { return v; }
 #endif
 };
+
+/* one thread on its own, on the device as on the host */
+struct InfOneLane {
+	DNG_HDI uint32_t lane() const { return 0; }
+	DNG_HDI uint32_t n() const { return 1; }
+	DNG_HDI void sync() const {}
+	DNG_HDI uint32_t bcast(uint32_t v, uint32_t) const { return v; }
+	DNG_HDI uint32_t ballot(bool v) const { return v; }
+};
+
+/* a split decode (inflate_split.cuh): a member's end, CRC-32 and ISIZE,
+ * checked once the pieces are joined */
+struct InfMember {
+	uint64_t end;		/* output offset of the member's end */
+	uint32_t crc, isize;
+};
+
+static const uint64_t INF_NOSTART = ~0ull;	/* a chunk without a candidate */
+static const uint32_t INF_NOLAND = ~0u;
 
 /* ---- CRC-32 (reflected, polynomial 0xedb88320) ------------------------- */
 
@@ -155,8 +180,8 @@ DNG_HDI uint32_t crc32_mulmod(uint32_t a, uint32_t b)
 	return p;
 }
 
-/* crc32(A || B) from crc32(A), crc32(B) and |B| */
-DNG_HDI uint32_t crc32_combine(uint32_t ca, uint32_t cb, uint64_t nb)
+/* x^(8 nb) modulo the polynomial: what appending nb bytes multiplies by */
+DNG_HDI uint32_t crc32_shift(uint64_t nb)
 {
 	uint32_t x = 1u << 30;		/* x^1: x^(2^k) as k steps */
 	uint32_t p = 1u << 31;		/* x^0 */
@@ -167,26 +192,91 @@ DNG_HDI uint32_t crc32_combine(uint32_t ca, uint32_t cb, uint64_t nb)
 		x = crc32_mulmod(x, x);
 		n >>= 1;
 	}
-	return crc32_mulmod(p, ca) ^ cb;
+	return p;
 }
 
-/* ---- the decoder ----------------------------------------------------------- */
+/* crc32(A || B) from crc32(A), crc32(B) and |B| */
+DNG_HDI uint32_t crc32_combine(uint32_t ca, uint32_t cb, uint64_t nb)
+{
+	return crc32_mulmod(crc32_shift(nb), ca) ^ cb;
+}
 
-struct Inflater {
+/* ---- the decoder -----------------------------------------------------------
+ *
+ * Sym is the output symbol: bytes (inflate_one), or 16-bit symbols for a
+ * decode that starts at a block inside a member (inflate_split.cuh), where a
+ * distance reaching before the start gives a marker, 256 + i for byte i of
+ * the 32 KiB before it.  Lanes: a warp, or one thread.  Tab: the decode
+ * tables; Tab::LBITS and Tab::DBITS size their fast tables (0: none).
+ */
+template <class Sym, class Lanes, class Tab>
+struct InflaterT {
 	const uint8_t *in;
 	uint64_t n;		/* compressed bytes */
 	uint64_t next;		/* next byte to load into bb */
 	uint64_t bb;		/* bit buffer, low bits first */
 	uint32_t bc;		/* bits in bb */
-	uint8_t *out;
+	Sym *out;
 	uint64_t cap, pos;
 	uint64_t mstart;	/* output offset of the current member */
 	uint32_t kind;
-	InfTables *T;
+	Tab *T;
 	const uint32_t *crct;
-	InfLanes L;
+	Lanes L;
+	/* a split decode: the member began before the output's start (markers);
+	 * the later chunks' candidate bits, where a block start ends the decode
+	 * (`land`: which one); the member ends, recorded instead of checked */
+	bool window;
+	const uint64_t *cand;
+	uint32_t ncand, ci, land;
+	InfMember *mem;
+	uint32_t mcap;
+
+	/* every field but the input, output and tables: a decode from bit 0 */
+	DNG_HDI void reset()
+	{
+		next = 0;
+		bb = 0;
+		bc = 0;
+		pos = 0;
+		mstart = 0;
+		kind = 0;
+		crct = nullptr;
+		window = false;
+		cand = nullptr;
+		ncand = ci = 0;
+		land = INF_NOLAND;
+		mem = nullptr;
+		mcap = 0;
+	}
 
 	DNG_HDI uint64_t bitpos() const { return next * 8 - bc; }
+
+	/* start reading at input bit `bit` (< 8 n) */
+	DNG_HDI void seek(uint64_t bit)
+	{
+		next = bit >> 3;
+		bb = 0;
+		bc = 0;
+		refill();
+		bb >>= bit & 7;
+		bc -= bit & 7;
+	}
+
+	/* a block starts here: is it a later chunk's candidate? */
+	DNG_HDI bool landed()
+	{
+		if (!cand)
+			return false;
+		const uint64_t b = bitpos();
+		while (ci < ncand && (cand[ci] < b || cand[ci] == INF_NOSTART))
+			ci++;
+		if (ci < ncand && cand[ci] == b) {
+			land = ci;
+			return true;
+		}
+		return false;
+	}
 
 	DNG_HDI void refill()
 	{
@@ -347,9 +437,9 @@ struct Inflater {
 			    i < 288 ? 8 : 5;
 		L.sync();
 		if (!build(T->lens, 288, T->lcount, T->loffs, T->lfirst, T->lsym,
-		    T->lfast, INF_LBITS, false) ||
+		    T->lfast, Tab::LBITS, false) ||
 		    !build(T->lens + 288, 32, T->dcount, T->doffs, T->dfirst,
-		    T->dsym, T->dfast, INF_DBITS, false))
+		    T->dsym, T->dfast, Tab::DBITS, false))
 			return false;
 		T->fixed = 1;	/* (every lane stores the same value) */
 		return true;
@@ -384,7 +474,7 @@ struct Inflater {
 				T->lens[288 + i] = cl[i];
 		L.sync();
 		if (!build(T->lens + 288, 19, T->dcount, T->doffs, T->dfirst,
-		    T->dsym, T->dfast, INF_DBITS, true))
+		    T->dsym, T->dfast, Tab::DBITS, true))
 			return false;
 		const uint32_t total = nlen + ndist;
 		uint32_t have = 0, prev = 0;
@@ -392,7 +482,7 @@ struct Inflater {
 		L.sync();
 		while (have < total) {
 			uint32_t s, rep, v = 0;
-			if (!decode(T->dcount, T->dsym, T->dfast, INF_DBITS, s))
+			if (!decode(T->dcount, T->dsym, T->dfast, Tab::DBITS, s))
 				return false;
 			if (s < 16) {
 				if (L.lane() == 0)
@@ -439,9 +529,9 @@ struct Inflater {
 			lens[288 + i] = i < 30 ? dl[i] : 0;
 		L.sync();
 		return build(lens, nlen, T->lcount, T->loffs, T->lfirst, T->lsym,
-		    T->lfast, INF_LBITS, false) &&
+		    T->lfast, Tab::LBITS, false) &&
 		    build(lens + 288, ndist, T->dcount, T->doffs, T->dfirst,
-		    T->dsym, T->dfast, INF_DBITS, false);
+		    T->dsym, T->dfast, Tab::DBITS, false);
 	}
 
 	/* 0: block ok, 1: out of room, else false via fail() */
@@ -460,13 +550,13 @@ struct Inflater {
 		    13, 13 };
 		for (;;) {
 			uint32_t s;
-			if (!decode(T->lcount, T->lsym, T->lfast, INF_LBITS, s))
+			if (!decode(T->lcount, T->lsym, T->lfast, Tab::LBITS, s))
 				return -1;
 			if (s < 256) {
 				if (pos >= cap)
 					return 1;
 				if (L.lane() == 0)
-					out[pos] = (uint8_t)s;
+					out[pos] = (Sym)s;
 				pos++;
 				continue;
 			}
@@ -479,20 +569,30 @@ struct Inflater {
 			if (!bits(lext[s], e))
 				return -1;
 			len = lbase[s] + e;
-			if (!decode(T->dcount, T->dsym, T->dfast, INF_DBITS, ds))
+			if (!decode(T->dcount, T->dsym, T->dfast, Tab::DBITS, ds))
 				return -1;
 			if (ds >= 30)
 				return fail(IE_CODE) ? 0 : -1;
 			if (!bits(dext[ds], e))
 				return -1;
 			dist = dbase[ds] + e;
-			if (dist > pos - mstart)
+			if (dist > pos - mstart && !window)
 				return fail(IE_DISTANCE) ? 0 : -1;
 			if (pos + len > cap)
 				return 1;
 			L.sync();	/* lane 0's literals, seen by every lane */
-			const uint8_t *src = out + pos - dist;
-			uint8_t *dst = out + pos;
+			Sym *dst = out + pos;
+			if (dist > pos) {
+				/* (only with a window) markers for what lies before */
+				const int64_t from = (int64_t)pos - dist;
+				for (uint32_t i = L.lane(); i < len; i += L.n()) {
+					const int64_t k = from + i % dist;
+					dst[i] = k >= 0 ? out[k] : (Sym)(256 + 32768 + k);
+				}
+				pos += len;
+				continue;
+			}
+			const Sym *src = out + pos - dist;
 			if (dist >= len) {
 				for (uint32_t i = L.lane(); i < len; i += L.n())
 					dst[i] = src[i];
@@ -561,8 +661,9 @@ struct Inflater {
 		return true;
 	}
 
-	/* one member's trailer; its output is [mstart, pos) */
-	DNG_HDI bool trailer()
+	/* one member's trailer; its output is [mstart, pos), or, in a split
+	 * decode, ends at pos and is recorded as member m */
+	DNG_HDI bool trailer(uint32_t m)
 	{
 		align();
 		uint32_t t[8];
@@ -571,6 +672,11 @@ struct Inflater {
 				return false;
 		const uint32_t want = t[0] | t[1] << 8 | t[2] << 16 | t[3] << 24;
 		const uint32_t isize = t[4] | t[5] << 8 | t[6] << 16 | t[7] << 24;
+		if (mem) {
+			if (L.lane() == 0)
+				mem[m] = { pos, want, isize };
+			return true;
+		}
 		/* each lane a piece of at least 4 KiB, combined in order */
 		L.sync();
 		const uint64_t total = pos - mstart;
@@ -579,8 +685,8 @@ struct Inflater {
 			piece = 4096;
 		const uint64_t lo = mstart + piece * L.lane();
 		const uint64_t hi = lo + piece < pos ? lo + piece : pos;
-		const uint32_t mine = lo < hi ? crc32_run(crct, out + lo, hi - lo) :
-		    0;
+		const uint32_t mine = lo < hi ?
+		    crc32_run(crct, (const uint8_t *)(out + lo), hi - lo) : 0;
 		uint32_t crc = 0;
 		for (uint32_t i = 0; i < L.n(); i++) {
 			const uint32_t c = L.bcast(mine, i);
@@ -596,7 +702,8 @@ struct Inflater {
 		return true;
 	}
 
-	/* the whole file */
+	/* the whole file; or, with a window, from a block inside a member to
+	 * the end, or to a block start that landed() */
 	DNG_HDI void run(InfResult &r)
 	{
 		r.status = INF_DONE;
@@ -605,15 +712,22 @@ struct Inflater {
 		r.bit = 0;
 		T->fixed = 0;
 		L.sync();
-		for (;;) {
-			while (r.members && next < n && in[next] == 0)
-				next++;
-			if (next >= n)
-				break;
-			if (!header())
-				goto error;
-			mstart = pos;
+		for (bool inside = window;; inside = false) {
+			if (!inside) {
+				while (r.members && next < n && in[next] == 0)
+					next++;
+				if (next >= n)
+					break;
+				if (!header())
+					goto error;
+				mstart = pos;
+				window = false;
+			}
 			for (;;) {
+				if (landed()) {
+					r.out_len = pos;
+					return;
+				}
 				uint32_t last, type;
 				if (!bits(1, last) || !bits(2, type))
 					goto error;
@@ -628,18 +742,21 @@ struct Inflater {
 					rc = fail(IE_BLOCK_TYPE) ? 0 : -1;
 				if (rc < 0)
 					goto error;
-				if (rc > 0) {
-					r.status = INF_ROOM;
-					r.out_len = pos;
-					return;
-				}
+				if (rc > 0)
+					goto room;
 				if (last)
 					break;
 			}
-			if (!trailer())
+			if (mem && r.members >= mcap)
+				goto room;	/* (no slot for the member) */
+			if (!trailer(r.members))
 				goto error;
 			r.members++;
 		}
+		r.out_len = pos;
+		return;
+	room:
+		r.status = INF_ROOM;
 		r.out_len = pos;
 		return;
 	error:
@@ -650,22 +767,19 @@ struct Inflater {
 	}
 };
 
+typedef InflaterT<uint8_t, InfLanes, InfTables> Inflater;
+
 /* decode in[0, in_len) into out[0, cap): the host's entry (one lane) and the
  * body of each warp of inflate_kernel */
 DNG_HDI void inflate_one(const InfJob &j, InfTables *T, const uint32_t *crct,
     InfResult &r)
 {
 	Inflater f;
+	f.reset();
 	f.in = j.in;
 	f.n = j.in_len;
-	f.next = 0;
-	f.bb = 0;
-	f.bc = 0;
 	f.out = j.out;
 	f.cap = j.cap;
-	f.pos = 0;
-	f.mstart = 0;
-	f.kind = 0;
 	f.T = T;
 	f.crct = crct;
 	f.run(r);

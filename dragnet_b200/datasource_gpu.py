@@ -149,6 +149,7 @@ def run_plan(plan, files=(), chunks=None, device=0, device_buffers=None,
             stats.update(s.read_stats())
             if gzip:
                 stats.update(s.gzip_stats())
+                stats.update(s.gzip_split_stats())
         pts = []
         if 'metrics' in plan:
             # fan-out: points are tagged like the reference tags them

@@ -98,6 +98,8 @@ _SIGS = [
     ('dng_scan_gzip_stats', ctypes.c_int,
      [_P] + [ctypes.POINTER(ctypes.c_uint64)] * 5 +
      [ctypes.POINTER(ctypes.c_double)]),
+    ('dng_scan_gzip_split_stats', ctypes.c_int,
+     [_P] + [ctypes.POINTER(ctypes.c_uint64)] * 5),
     ('dng_scan_launch_count', ctypes.c_uint64, [_P]),
     ('dng_pinned_alloc', _P, [ctypes.c_size_t]),
     ('dng_pinned_free', None, [_P]),
@@ -176,6 +178,8 @@ JIT_CACHE_STATS = ['hits', 'misses', 'writes', 'evictions', 'errors']
 READ_STATS = ['direct_bytes', 'buffered_bytes', 'direct_ranges', 'fallbacks']
 GZIP_STATS = ['gzip_files', 'gzip_members', 'gzip_compressed_bytes',
               'gzip_inflated_bytes', 'inflate_launches', 'inflate_ms']
+GZIP_SPLIT_STATS = ['gzip_split_files', 'gzip_chunks', 'gzip_false_starts',
+                    'gzip_fallbacks', 'gzip_split_launches']
 
 
 def set_jit_cache_dir(path):
@@ -403,6 +407,16 @@ class _ScanStats(object):
                                          *[ctypes.byref(x) for x in v],
                                          ctypes.byref(ms)), self.handle)
         return dict(zip(GZIP_STATS, [int(x.value) for x in v] + [ms.value]))
+
+    def gzip_split_stats(self):
+        """The split path of dng_scan_feed_gzip: files cut into chunks,
+        chunks, false starts among their candidates, files decoded whole
+        after the split path could not vouch for them, split kernel
+        launches."""
+        v = [ctypes.c_uint64() for _ in GZIP_SPLIT_STATS]
+        _check(lib().dng_scan_gzip_split_stats(
+            self.handle, *[ctypes.byref(x) for x in v]), self.handle)
+        return dict(zip(GZIP_SPLIT_STATS, (int(x.value) for x in v)))
 
 
 class Scan(_ScanStats):

@@ -189,11 +189,22 @@ int dng_scan_sync(dng_scan *scan);
  */
 int dng_scan_feed_gzip(dng_scan *scan, const char *path);
 /* Gzip files inflated so far, their members, compressed and decompressed
- * bytes, inflate kernel launches (one per batch, plus one per decode of a
- * file again in more room) and their time (CUDA events). */
+ * bytes, inflate kernel launches (one per batch that has a file decoded by
+ * one warp, plus one per decode of a file again in more room, or whole after
+ * the split path could not vouch for it) and the time of every inflate
+ * kernel, the split path's included (CUDA events). */
 int dng_scan_gzip_stats(dng_scan *scan, uint64_t *files, uint64_t *members,
     uint64_t *compressed_bytes, uint64_t *inflated_bytes, uint64_t *launches,
     double *inflate_ms);
+/* The split path: a large file in a batch of fewer files than the device
+ * holds decode warps is cut into chunks at block starts found on the device
+ * and decoded by one warp per chunk.  Files split, their chunks, candidate
+ * block starts nothing landed on (false starts), files decoded whole after
+ * the split path could not vouch for them (fallbacks: damaged files only),
+ * and the split kernels' launches (also in dng_scan_launch_count). */
+int dng_scan_gzip_split_stats(dng_scan *scan, uint64_t *split_files,
+    uint64_t *chunks, uint64_t *false_starts, uint64_t *fallbacks,
+    uint64_t *launches);
 
 /* End of input: flushes the final unterminated line, then emits the points. */
 int dng_scan_finish(dng_scan *scan, dng_result **out);

@@ -10,7 +10,7 @@ mkdir -p build/var_$1
 /usr/local/cuda/bin/nvcc -O3 -std=c++17 -lineinfo -gencode arch=compute_90a,code=sm_90a \
     -Xcompiler -fPIC,-Wall $2 -Xptxas -v -c -o build/var_$1/api.o api.cu 2> build/var_$1/api.log
 grep -A2 "scan_kernelENS" build/var_$1/api.log | grep -E "registers|spill" || true
-make -s build/merge.o build/plan.o build/result.o build/tmpl.o build/fast.o build/jit.o build/jit_load.o build/jit_blob.o
+make -s build/merge.o build/plan.o build/result.o build/tmpl.o build/fast.o build/jit.o build/jit_load.o build/jit_cache.o build/jit_blob.o
 /usr/local/cuda/bin/nvcc -gencode arch=compute_90a,code=sm_90a -shared \
     -o ../libdragnet_gpu_$1.so build/var_$1/api.o build/merge.o build/plan.o build/result.o build/tmpl.o \
-    build/fast.o build/jit.o build/jit_load.o build/jit_blob.o -ldl
+    build/fast.o build/jit.o build/jit_load.o build/jit_cache.o build/jit_blob.o -ldl
