@@ -319,6 +319,36 @@ int upload_blob(dng_scan *s, int half, std::vector<u8> &blob, u8 **dst)
 }
 
 /*
+ * Do the accepted templates' sample lines all have short group keys (fast.cuh
+ * FKey)?  What the compiled kernel keeps in its record loop depends on it
+ * (FPlan::short_keys); what it counts does not.
+ */
+static bool fsample_keys_short(const FPlan &F,
+    const std::vector<TResolved> &fres, const std::vector<u8> &accepted)
+{
+	if (F.ncols > FK_COLS)
+		return false;
+	for (size_t i = 0; i < fres.size(); i++) {
+		if (!accepted[i])
+			continue;
+		for (u32 j = 0; j < F.ncols; j++) {
+			const Col &col = F.col[j];
+			if (col.kind != COL_DISCRETE)
+				continue;
+			/* (undefined is 9 bytes) */
+			if (col.src.kind != SRC_PATH ||
+			    !((fres[i].set_mask >> col.src.idx) & 1))
+				return false;
+			const u64 v = fres[i].slots[col.src.idx];
+			const u32 t = val_type(v);
+			if ((t == T_STR || t == T_NUM) && val_len(v) > FK_W)
+				return false;
+		}
+	}
+	return true;
+}
+
+/*
  * The F path's templates (fast.h): the same candidates, their captures indexed
  * by path, compact literals.  `blob` keeps them for the compiled matcher, `t`
  * says what they cover of the sample.
@@ -333,6 +363,8 @@ int learn_ftemplates(dng_scan *s, const std::vector<TCandidate> &cands,
 	std::vector<u8> accepted;
 	u32 nt = 0;
 	tmpl_build(cands, fres, TMPL_RESERVE, blob, &nt, true, &accepted);
+	s->fplan.short_keys = !blob.empty() &&
+	    fsample_keys_short(s->fplan, fres, accepted);
 	cached_free(s->d_ftmpl);
 	s->d_ftmpl = nullptr;
 	s->ftmpl_bytes = 0;

@@ -393,6 +393,39 @@ DNG_PLAN_LOOP
 }
 
 /*
+ * The short key: a group key of at most FK_COLS columns whose discrete pieces
+ * are at most FK_W bytes, packed into registers at a fixed layout so that it
+ * is hashed, compared and stored a word at a time.  Column j owns w[2j] and
+ * w[2j + 1]: a discrete piece's bytes, zero padded, or an ordinal's binary64.
+ * hdr = FK_PACKED | ncols << 16 | one nibble per column at bit 4j: a discrete
+ * piece's length, or FK_ORD for an ordinal; 0 = the key does not fit.
+ *
+ * Equal short keys are equal keys: every byte of record.cuh's encoding is in
+ * hdr or w.  Whether a key fits depends only on its content, so one key
+ * always takes the same form; a slot stores the short form with hdr in place
+ * of klen (bit 31: never a length), and the F kernel's flush turns it back
+ * into the encoding (fkey_unpack) before it leaves the CTA.
+ */
+enum : u32 { FK_COLS = 4, FK_W = 8, FK_WORDS = 2 * FK_COLS, FK_ORD = 0xf,
+	FK_PACKED = 0x80000000u };
+struct FKey {
+	u32 hdr;
+	u32 w[FK_WORDS];
+};
+
+/* w[2j], w[2j + 1] = lo, hi: static indexes only, so that w stays in
+ * registers when j is not a constant (the rolled loops of the ahead-of-time
+ * build) */
+DNG_HD void fkey_set(FKey &k, u32 j, u32 lo, u32 hi)
+{
+#pragma unroll
+	for (u32 i = 0; i < FK_COLS; i++) {
+		k.w[2 * i] = i == j ? lo : k.w[2 * i];
+		k.w[2 * i + 1] = i == j ? hi : k.w[2 * i + 1];
+	}
+}
+
+/*
  * The group key (record.cuh process_metric's encoding), column by column:
  * discrete = u16 length + the bytes of String(value), taken from the record
  * or from the plan's constants; bucketized = 0xFFFF + the ordinal's binary64.
@@ -400,12 +433,23 @@ DNG_PLAN_LOOP
  * fprep() looks at every column once: false = the F path does not build this
  * key (miss).  Ordinals are computed here and parked in two capture rows of
  * their own (FPlan::ord_row), so that hashing, comparing and writing the key
- * are cheap, cannot fail and agree with each other.
+ * are cheap, cannot fail and agree with each other.  The same pass fills the
+ * short key k (k.hdr = 0 when the key does not fit it).
  */
 template <class M>
 DNG_HD bool fprep(M &m, const FPlan &F, u32 defmask, double s0, double s1,
-    u32 &slow)
+    u32 &slow, FKey &k)
 {
+	u32 hdr = F.ncols <= FK_COLS ? FK_PACKED | (u32)F.ncols << 16 : 0;
+#ifdef DNG_JIT_HOT
+	/* (a plan constant there: without it the record loop is the piece-wise
+	 * code alone) */
+	if (!F.short_keys)
+		hdr = 0;
+#endif
+#pragma unroll
+	for (u32 i = 0; i < FK_WORDS; i++)
+		k.w[i] = 0;
 DNG_PLAN_LOOP
 	for (u32 j = 0; j < F.ncols; j++) {
 		const Col &col = F.col[j];
@@ -421,6 +465,28 @@ DNG_PLAN_LOOP
 			 * of a date: the general path */
 			if (synth || (t == T_NUM && !fcap_flag(cw)))
 				return false;
+			/* String(value): the record's bytes (a string, a simple
+			 * integer) or "null", "true", "false", "undefined" */
+			const bool rec = t == T_STR || t == T_NUM;
+			const u32 n = rec ? fcap_len(cw) : t == T_UNDEF ? 9 :
+			    t == T_FALSE ? 5 : 4;
+			if (!hdr || n > FK_W) {
+				hdr = 0;
+				continue;
+			}
+			u32 lo, hi;
+			if (rec) {
+				m.words2(fcap_off(cw), lo, hi);
+				lo &= n >= 4 ? ~0u : (1u << (8 * n)) - 1;
+				hi &= n >= 8 ? ~0u : n <= 4 ? 0 :
+				    (1u << (8 * (n - 4))) - 1;
+			} else {
+				lo = t == T_NULL ? 0x6c6c756eu : t == T_TRUE ?
+				    0x65757274u : 0x736c6166u;
+				hi = t == T_FALSE ? 0x65u : 0;
+			}
+			hdr |= n << (4 * j);
+			fkey_set(k, j, lo, hi);
 			continue;
 		}
 		double x;
@@ -439,8 +505,49 @@ DNG_PLAN_LOOP
 		    double_to_bits(ord);
 		m.setcap(F.ord_row[j], (u32)b);
 		m.setcap(F.ord_row[j] + 1u, (u32)(b >> 32));
+		if (hdr) {
+			hdr |= FK_ORD << (4 * j);
+			fkey_set(k, j, (u32)b, (u32)(b >> 32));
+		}
 	}
+	k.hdr = hdr;
 	return true;
+}
+
+template <class M>
+DNG_HD bool fprep(M &m, const FPlan &F, u32 defmask, double s0, double s1,
+    u32 &slow)
+{
+	FKey k;
+	return fprep(m, F, defmask, s0, s1, slow, k);
+}
+
+/* the short key k in record.cuh's encoding (fkey_write's bytes), zero padded
+ * to a multiple of 8; returns its length.  out has room for 8 * FK_COLS + 8;
+ * k may live in the bytes it is written to. */
+DNG_HD u32 fkey_unpack(FKey k, u8 *out)
+{
+	const u32 ncols = (k.hdr >> 16) & 0xf;
+	u32 o = 0;
+#pragma unroll
+	for (u32 j = 0; j < FK_COLS; j++) {
+		if (j >= ncols)
+			break;
+		const u32 n = (k.hdr >> (4 * j)) & 0xf;
+		const u32 nb = n == FK_ORD ? 8 : n;
+		out[o] = n == FK_ORD ? 0xff : (u8)n;
+		out[o + 1] = n == FK_ORD ? 0xff : 0;
+#pragma unroll
+		for (u32 b = 0; b < FK_W; b++)
+			if (b < nb)
+				out[o + 2 + b] = (u8)(k.w[2 * j + b / 4] >>
+				    (8 * (b & 3)));
+		o += 2 + nb;
+	}
+	const u32 len = o;
+	while (o & 7)
+		out[o++] = 0;
+	return len;
 }
 
 struct FPiece {
@@ -481,6 +588,21 @@ DNG_HD u32 fmix(u32 h, u32 w)
 {
 	h = (h ^ w) * 0x9E3779B1u;
 	return h ^ (h >> 15);
+}
+
+/* the short key's hash: its header, then its columns' words (ncols =
+ * F.ncols: a constant of the link-time optimised build) */
+DNG_HD u32 fkey_short_hash(const FKey &k, u32 ncols)
+{
+	u32 h = fmix(0x2545F491u, k.hdr);
+#pragma unroll
+	for (u32 j = 0; j < FK_COLS; j++)
+		if (j < ncols)
+			h = fmix(fmix(h, k.w[2 * j]), k.w[2 * j + 1]);
+	h ^= h >> 16;
+	h *= 0x85ebca6bu;
+	h ^= h >> 13;
+	return h;
 }
 
 /* a piece's bytes as words from its start (the last one zero padded): the
@@ -648,6 +770,11 @@ struct FastHostMem : TmplHostMem {
 	u32 litw(u32 off) const { return pool32(off); }
 	void setcap(u32 p, u32 v) { caps[p] = v; }
 	u32 getcap(u32 p) const { return caps[p]; }
+	void words2(u32 off, u32 &lo, u32 &hi) const
+	{
+		lo = word(off);
+		hi = word(off + 4);
+	}
 };
 struct FastHostKey {
 	const u8 *key;

@@ -16,8 +16,10 @@
  *     stores the winning value (one 32-bit word per path, in shared memory);
  *   - the stages (lib/stream-scan.js:56-86: datasource filter, user filter,
  *     synthetic dates, time bounds, group key) evaluated straight from those
- *     captures, the key hashed and compared piece by piece in place -- it is
- *     only materialised the first time a CTA sees it.
+ *     captures; a short key (fast.cuh FKey: up to four columns, pieces of up
+ *     to 8 bytes) is packed into registers and hashed, compared and stored as
+ *     words, any other key is hashed and compared piece by piece in place --
+ *     it is only materialised the first time a CTA sees it.
  *
  * A record the F path cannot decide EXACTLY (no template, an escaped string
  * or a container where a value is needed, a key too long ...) is a "miss":
@@ -65,7 +67,13 @@ struct alignas(16) FPlan {
 					 * capture rows ord_row[j], + 1 */
 	u8 nrows;			/* capture rows in all */
 	u8 ncode;			/* leaves in code[]; jumps only go forward */
-	u8 pad[4];
+	u8 short_keys;			/* the templates' sample lines all have short
+					 * keys (fast.cuh FKey): the link-time
+					 * optimised kernel packs keys and calls the
+					 * piece-wise key code out of line; without
+					 * it, that kernel keys piece by piece only
+					 * (a hint: every way is exact for any key) */
+	u8 pad[3];
 	char pool[F_POOL];
 };
 

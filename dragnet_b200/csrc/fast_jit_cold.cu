@@ -26,5 +26,11 @@ extern "C" __device__ void dng_cold_miss(const u8 *data,
 extern "C" __device__ void dng_cold_flush(STab stab, u32 s1slots, u32 sslots,
     const GTable *tab)
 {
-	flush_tally(stab, s1slots, sslots, *tab);
+	fflush_tally(stab, s1slots, sslots, *tab);
+}
+
+extern "C" __device__ bool dng_cold_long_tally(FSmem m, const FPlan *F,
+    u32 defmask, STab stab, const GTable *gt, u32 over_sa)
+{
+	return flong_tally(m, *F, F, defmask, stab, *gt, over_sa);
 }

@@ -167,6 +167,18 @@ __device__ __forceinline__ void sts32(u32 addr, u32 v)
 	asm volatile("st.shared.u32 [%0], %1;" :: "r"(addr), "r"(v) : "memory");
 }
 
+__device__ __forceinline__ void sts64(u32 addr, unsigned long long v)
+{
+	asm volatile("st.shared.u64 [%0], %1;" :: "r"(addr), "l"(v) : "memory");
+}
+
+__device__ __forceinline__ unsigned long long lds64(u32 addr)
+{
+	unsigned long long v;
+	asm volatile("ld.shared.u64 %0, [%1];" : "=l"(v) : "r"(addr) : "memory");
+	return v;
+}
+
 /* shared-memory access for fmatch()/fstage()/fkey_*() */
 struct FSmem {
 	u32 ra;			/* record start (shared address) */
@@ -207,6 +219,19 @@ struct FSmem {
 		return c.wa - 4 - ra;
 	}
 	__device__ __forceinline__ u32 byte(u32 off) const { return lds8(ra + off); }
+	/* the 8 bytes from off: the two aligned 8-byte words around them (the
+	 * window is 8-byte aligned, and its slack follows it) */
+	__device__ __forceinline__ void words2(u32 off, u32 &lo, u32 &hi) const
+	{
+		const u32 a = ra + off;
+		const unsigned long long q0 = lds64(a & ~7u);
+		const unsigned long long q1 = lds64((a & ~7u) + 8);
+		const u32 sh = (a & 7) * 8;
+		const unsigned long long v = sh ? (q0 >> sh) | (q1 << (64 - sh)) :
+		    q0;
+		lo = (u32)v;
+		hi = (u32)(v >> 32);
+	}
 	__device__ __forceinline__ u32 word(u32 off) const
 	{
 		Cur c = cursor(off);
@@ -266,6 +291,8 @@ extern "C" __device__ void dng_cold_miss(const u8 *data,
     unsigned long long *counters);
 extern "C" __device__ void dng_cold_flush(STab stab, u32 s1slots, u32 sslots,
     const GTable *tab);
+extern "C" __device__ bool dng_cold_long_tally(FSmem m, const FPlan *F,
+    u32 defmask, STab stab, const GTable *gt, u32 over_sa);
 /*
  * The scan's plan as a CONSTANT of the generated code (jit.cpp writes it out
  * with its initialiser): after link-time optimisation the stage and key code
@@ -302,6 +329,15 @@ __device__ __forceinline__ void sts64_release(u32 addr, unsigned long long v)
 {
 	asm volatile("st.release.cta.shared.u64 [%0], %1;" :: "r"(addr), "l"(v)
 	    : "memory");
+}
+
+/* a key the inline tier has no room for (counted: the host gives the cache
+ * more room if this is common) */
+__device__ __forceinline__ void fover(FSmem &m, const FPlan *Fcold,
+    u32 defmask, u32 klen, const STab &stab, const GTable &gt, u32 over_sa)
+{
+	asm volatile("red.shared.add.u32 [%0], 1;" :: "r"(over_sa) : "memory");
+	fslow_add(m, Fcold, defmask, klen, stab, &gt);
 }
 
 /*
@@ -348,9 +384,110 @@ __device__ __forceinline__ void ftally(FSmem &m, const FPlan &F,
 			idx = (idx + 1) & stab.mask1;
 		}
 	}
-	/* (counted: the host gives the cache more room if this is common) */
-	asm volatile("red.shared.add.u32 [%0], 1;" :: "r"(over_sa) : "memory");
-	fslow_add(m, Fcold, defmask, klen, stab, &gt);
+	fover(m, Fcold, defmask, klen, stab, gt, over_sa);
+}
+
+/*
+ * Count a short key (fast.cuh FKey): the same inline tier, probed with the
+ * short key's hash; the slot holds k.hdr for klen and k.w as its key, read
+ * and written 8 bytes at a time at their fixed places.  A key the tier has no
+ * room for takes the general path in record.cuh's encoding.
+ */
+__device__ __forceinline__ void ftally_short(FSmem &m, const FPlan &F,
+    const FPlan *Fcold, u32 defmask, const FKey &k, const STab &stab,
+    const GTable &gt, u32 over_sa)
+{
+	const u32 h = fkey_short_hash(k, F.ncols);
+	const unsigned long long claim = (unsigned long long)(h | 1u);
+	u32 idx = (h >> 7) & stab.mask1;
+	for (u32 probe = 0; probe < 8; probe++) {
+		SSlot1 *s = &stab.s1[idx];
+		const u32 sa = smem_u32(s);
+		const u32 ka = sa + (u32)offsetof(SSlot1, key);
+		unsigned long long tag = lds64_acquire(sa);
+		if (tag == 0) {
+			const unsigned long long old = atomicCAS(&s->tag, 0ull,
+			    claim);
+			if (old == 0) {
+				sts32(sa + (u32)offsetof(SSlot1, klen), k.hdr);
+#pragma unroll
+				for (u32 j = 0; j < FK_COLS; j++)
+					if (j < F.ncols)
+						sts64(ka + 8 * j, k.w[2 * j] |
+						    (unsigned long long)
+						    k.w[2 * j + 1] << 32);
+				atomicAdd(&s->count, 1u);
+				sts64_release(sa, claim | DNG_READY);
+				return;
+			}
+			tag = old;
+		}
+		if ((tag & ~DNG_READY) == claim) {
+			while (!(tag & DNG_READY))
+				tag = lds64_acquire(sa);
+			unsigned long long diff = lds32(sa +
+			    (u32)offsetof(SSlot1, klen)) ^ k.hdr;
+#pragma unroll
+			for (u32 j = 0; j < FK_COLS; j++)
+				if (j < F.ncols)
+					diff |= lds64(ka + 8 * j) ^ (k.w[2 * j] |
+					    (unsigned long long)k.w[2 * j + 1] << 32);
+			if (diff == 0) {
+				atomicAdd(&s->count, 1u);
+				return;
+			}
+		}
+		idx = (idx + 1) & stab.mask1;
+	}
+	/* (the key's length in record.cuh's encoding) */
+	u32 klen = 0;
+#pragma unroll
+	for (u32 j = 0; j < FK_COLS; j++) {
+		const u32 n = (k.hdr >> (4 * j)) & 0xf;
+		if (j < F.ncols)
+			klen += n == FK_ORD ? 10 : 2 + n;
+	}
+	fover(m, Fcold, defmask, klen, stab, gt, over_sa);
+}
+
+/* the F kernel's end: its short keys in record.cuh's encoding, then the
+ * common flush (flush_tally) */
+__device__ __forceinline__ void fflush_tally(const STab &stab, u32 s1slots,
+    u32 sslots, const GTable &tab)
+{
+	__syncthreads();
+	for (u32 i = threadIdx.x; i < s1slots; i += blockDim.x) {
+		SSlot1 *s = &stab.s1[i];
+		if (s->tag == 0 || !(s->klen & FK_PACKED))
+			continue;
+		FKey k;
+		k.hdr = s->klen;
+#pragma unroll
+		for (u32 j = 0; j < FK_COLS; j++) {
+			k.w[2 * j] = (u32)s->key[j];
+			k.w[2 * j + 1] = (u32)(s->key[j] >> 32);
+		}
+		s->klen = fkey_unpack(k, (u8 *)s->key);
+	}
+	flush_tally(stab, s1slots, sslots, tab);
+}
+
+/*
+ * A key that is not a short key: hashed, compared and tallied piece by piece
+ * (false: longer than the F path carries).  Where the templates' samples have
+ * only short keys (FPlan::short_keys) the link-time optimised kernel calls it
+ * out of line (dng_cold_long_tally): the H100's instruction cache does not
+ * hold its code in the record loop as well as the short key's.
+ */
+__device__ __forceinline__ bool flong_tally(FSmem &m, const FPlan &F,
+    const FPlan *Fcold, u32 defmask, const STab &stab, const GTable &gt,
+    u32 over_sa)
+{
+	u32 h, klen;
+	if (!fkey_hash(m, F, defmask, h, klen))
+		return false;
+	ftally(m, F, Fcold, defmask, h, klen, stab, gt, over_sa);
+	return true;
 }
 
 #ifndef DNG_JIT_HOT
@@ -712,17 +849,31 @@ __device__ __forceinline__ void fscan_body(const FScanArgs &a)
 				if (matched) {
 					double s0, s1;
 					fo = fstage(m, F, defmask, s0, s1);
-					u32 h = 0, klen = 0, slow = 0;
-					if (fo == FO_AGGR && (!fprep(m, F, defmask,
-					    s0, s1, slow) || !fkey_hash(m, F,
-					    defmask, h, klen)))
+					u32 slow = 0;
+					FKey k;
+					if (fo == FO_AGGR && !fprep(m, F, defmask, s0,
+					    s1, slow, k))
 						fo = FO_MISS;
 					if (fo == FO_AGGR) {
-						if (slow)
+						if (k.hdr)
+							ftally_short(m, F,
+							    (const FPlan *)smem,
+							    defmask, k, stab, a.tab,
+							    smem_u32(&s_drop[15]));
+						else if (!(
+#ifdef DNG_JIT_HOT
+						    F.short_keys ?
+						    dng_cold_long_tally(m,
+						    (const FPlan *)smem, defmask,
+						    stab, &a.tab,
+						    smem_u32(&s_drop[15])) :
+#endif
+						    flong_tally(m, F, (const FPlan *)
+						    smem, defmask, stab, a.tab,
+						    smem_u32(&s_drop[15]))))
+							fo = FO_MISS;
+						if (fo == FO_AGGR && slow)
 							atomicAdd(&s_drop[1], 1u);
-						ftally(m, F, (const FPlan *)smem, defmask,
-						    h, klen, stab, a.tab,
-						    smem_u32(&s_drop[15]));
 					}
 				}
 				const bool done = fo != FO_MISS;
@@ -791,7 +942,7 @@ __device__ __forceinline__ void fscan_body(const FScanArgs &a)
 	__syncthreads();
 	dng_cold_flush(stab, a.s1slots, a.sslots, &a.tab);
 #else
-	flush_tally(stab, a.s1slots, a.sslots, a.tab);
+	fflush_tally(stab, a.s1slots, a.sslots, a.tab);
 #endif
 	if (lane == 0) {
 		if (ntmpl) {

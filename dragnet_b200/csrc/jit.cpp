@@ -203,7 +203,7 @@ static void plan_source(const FPlan &F, std::string &s)
 	    "struct Col { u64 step; Src src; u8 kind; u8 pad[5]; };\n"
 	    "struct alignas(16) FPlan { Leaf code[16]; Col col[6]; "
 	    "u8 syn_path[2]; short ds_entry, user_entry, time_entry; "
-	    "u8 nsyn, ncols, npaths, ok; u8 ord_row[6]; u8 nrows, ncode; u8 pad[4]; "
+	    "u8 nsyn, ncols, npaths, ok; u8 ord_row[6]; u8 nrows, ncode, short_keys; u8 pad[3]; "
 	    "char pool[512]; };\n";
 	appendf(s, "static_assert(sizeof (Leaf) == %zu && sizeof (Col) == %zu && "
 	    "sizeof (FPlan) == %zu, \"plan layout\");\n", sizeof (Leaf),
@@ -233,11 +233,11 @@ static void plan_source(const FPlan &F, std::string &s)
 	    (unsigned)F.syn_path[0], (unsigned)F.syn_path[1], (int)F.ds_entry,
 	    (int)F.user_entry, (int)F.time_entry, (unsigned)F.nsyn,
 	    (unsigned)F.ncols, (unsigned)F.npaths, (unsigned)F.ok);
-	appendf(s, "	{ %u, %u, %u, %u, %u, %u }, %u, %u, { 0, 0, 0, 0 },\n	{ ",
+	appendf(s, "	{ %u, %u, %u, %u, %u, %u }, %u, %u, %u, { 0, 0, 0 },\n	{ ",
 	    (unsigned)F.ord_row[0], (unsigned)F.ord_row[1],
 	    (unsigned)F.ord_row[2], (unsigned)F.ord_row[3],
 	    (unsigned)F.ord_row[4], (unsigned)F.ord_row[5], (unsigned)F.nrows,
-	    (unsigned)F.ncode);
+	    (unsigned)F.ncode, (unsigned)F.short_keys);
 	for (int i = 0; i < F_POOL; i++)
 		appendf(s, "%d,%s", (int)(signed char)F.pool[i],
 		    i % 32 == 31 ? "\n	  " : "");
