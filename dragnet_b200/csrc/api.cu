@@ -38,6 +38,8 @@
 #include "inflate.cuh"
 #include "inflate_policy.h"
 #include "inflate_split.cuh"
+#include "bunzip.cuh"
+#include "bunzip_policy.h"
 
 using namespace dng;
 
@@ -177,18 +179,22 @@ struct dng_scan {
 	/* dng_scan_read_stats */
 	uint64_t direct_bytes = 0, buffered_bytes = 0, direct_ranges = 0;
 	uint64_t read_fallbacks = 0;
-	/* dng_scan_feed_gzip: files queued for the next inflate batch (path,
-	 * compressed size, output room), the batch's device buffers, stats */
-	struct GzFile {
+	/* dng_scan_feed_gzip and dng_scan_feed_bzip2: compressed files queued
+	 * for the next batch, all of one format (path, compressed size, output
+	 * room of a gzip file), and the batch's compressed bytes */
+	struct CzFile {
 		std::string path;
 		size_t size;
 		uint64_t hint;
+		uint32_t head;		/* a bzip2 file's first four bytes */
 	};
-	std::vector<GzFile> gz_queue;
-	uint64_t gz_queued_in = 0, gz_queued_out = 0;
-	u8 *d_gz_in = nullptr, *d_gz_out = nullptr, *d_gz_big = nullptr;
+	std::vector<CzFile> cz_queue;
+	bool cz_bzip2 = false;		/* the queue's format */
+	uint64_t cz_queued_in = 0, cz_queued_out = 0;
+	/* the gzip path's device buffers and stats */
+	u8 *d_cz_in = nullptr, *d_gz_out = nullptr, *d_gz_big = nullptr;
 	u8 *d_gz_join = nullptr;
-	size_t gz_in_cap = 0, gz_out_cap = 0, gz_big_cap = 0, gz_join_cap = 0;
+	size_t cz_in_cap = 0, gz_out_cap = 0, gz_big_cap = 0, gz_join_cap = 0;
 	u8 *d_gz_jobs = nullptr, *h_gz_jobs = nullptr;	/* jobs, results, next */
 	uint64_t gz_files = 0, gz_members = 0, gz_in_bytes = 0, gz_out_bytes = 0;
 	uint64_t gz_launches = 0;
@@ -202,6 +208,17 @@ struct dng_scan {
 	uint64_t gz_split_files = 0, gz_chunks = 0, gz_false_starts = 0;
 	uint64_t gz_fallbacks = 0, gz_split_launches = 0;
 	uint32_t gz_split_blocks = 0;	/* CTAs of split_decode_kernel per SM */
+	/* the bzip2 path (bunzip.cuh): candidates, BWT slots, transformation
+	 * vectors, per-block records and output of a wave; its stats */
+	u8 *d_bz_find = nullptr, *d_bz_slot = nullptr, *d_bz_tt = nullptr;
+	u8 *d_bz_rec = nullptr, *d_bz_out = nullptr;
+	size_t bz_find_cap = 0, bz_slot_cap = 0, bz_tt_cap = 0, bz_rec_cap = 0;
+	size_t bz_out_cap = 0;
+	uint64_t bz_files = 0, bz_streams = 0, bz_blocks = 0;
+	uint64_t bz_false_starts = 0, bz_in_bytes = 0, bz_out_bytes = 0;
+	uint64_t bz_launches = 0;
+	double bz_ms = 0;
+	double bz_stage_ms[4] = {};	/* find, decode, invert, emit */
 	/* stats */
 	std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_pairs;
 	std::vector<cudaEvent_t> ev_pool;
@@ -1127,7 +1144,7 @@ int dng_scan_set_stream(dng_scan *s, void *cuda_stream)
 	return DNG_OK;
 }
 
-static int gz_flush(dng_scan *s);
+static int cz_flush(dng_scan *s);
 static int feed_device(dng_scan *s, const void *devbuf, size_t len);
 
 static int ensure_ring(dng_scan *s, bool need_stage)
@@ -1154,7 +1171,7 @@ int dng_scan_feed(dng_scan *s, const void *buf, size_t len)
 	if (s->multi)
 		return refuse_multi(s, "dng_scan_feed");
 	cudaSetDevice(s->device);
-	if (gz_flush(s) || ensure_ring(s, true))
+	if (cz_flush(s) || ensure_ring(s, true))
 		return s->err_code;
 	return feed_host(s, buf, len, false);
 }
@@ -1166,7 +1183,7 @@ int dng_scan_feed_pinned(dng_scan *s, const void *buf, size_t len)
 	if (s->multi)
 		return refuse_multi(s, "dng_scan_feed_pinned");
 	cudaSetDevice(s->device);
-	if (gz_flush(s) || ensure_ring(s, false))
+	if (cz_flush(s) || ensure_ring(s, false))
 		return s->err_code;
 	return feed_host(s, buf, len, true);
 }
@@ -1598,7 +1615,7 @@ int dng_scan_feed_file(dng_scan *s, const char *path)
 	if (s->multi)
 		return record_file(s, path);
 	cudaSetDevice(s->device);
-	if (gz_flush(s) || ensure_ring(s, false))
+	if (cz_flush(s) || ensure_ring(s, false))
 		return s->err_code;
 	int fd = open(path, O_RDONLY);
 	if (fd < 0)
@@ -1621,7 +1638,7 @@ int dng_scan_feed_device(dng_scan *s, const void *devbuf, size_t len)
 	if (s->multi)
 		return refuse_multi(s, "dng_scan_feed_device");
 	cudaSetDevice(s->device);
-	if (gz_flush(s))
+	if (cz_flush(s))
 		return s->err_code;
 	return feed_device(s, devbuf, len);
 }
@@ -1952,7 +1969,7 @@ static int gz_split_decode(dng_scan *s, std::vector<GzChunk> &ck,
 
 /* 1 and 2: enqueue the finder and the first decode of every chunk of the
  * split files (no wait) */
-static int gz_split_start(dng_scan *s, const std::vector<dng_scan::GzFile> &q,
+static int gz_split_start(dng_scan *s, const std::vector<dng_scan::CzFile> &q,
     const std::vector<size_t> &in_off, const std::vector<u32> &nch,
     std::vector<GzSplitFile> &sf, std::vector<GzChunk> &ck, GzTimer &t)
 {
@@ -1970,13 +1987,13 @@ static int gz_split_start(dng_scan *s, const std::vector<dng_scan::GzFile> &q,
 	}
 	ck.resize(total);
 	for (const GzSplitFile &f : sf) {
-		const dng_scan::GzFile &g = q[f.file];
+		const dng_scan::CzFile &g = q[f.file];
 		for (uint32_t k = 0; k < f.n; k++) {
 			const uint64_t cb = split_cut(g.size, f.n, k + 1) -
 			    split_cut(g.size, f.n, k);
 			SplitJob &j = ck[f.first + k].job;
 			j = {};
-			j.in = s->d_gz_in + in_off[f.file];
+			j.in = s->d_cz_in + in_off[f.file];
 			j.in_len = g.size;
 			j.cap = split_room(g.hint, g.size, cb);
 			j.k = k;
@@ -1998,7 +2015,7 @@ static int gz_split_start(dng_scan *s, const std::vector<dng_scan::GzFile> &q,
 	std::vector<SplitFind> finds;
 	uint64_t sym = 0;
 	for (const GzSplitFile &f : sf) {
-		const dng_scan::GzFile &g = q[f.file];
+		const dng_scan::CzFile &g = q[f.file];
 		for (uint32_t k = 0; k < f.n; k++) {
 			SplitJob &j = ck[f.first + k].job;
 			j.cand = d_cand + f.first;
@@ -2060,7 +2077,7 @@ static int gz_split_collect(dng_scan *s, std::vector<GzChunk> &ck,
  * members (alt[i]: where its bytes are when not in its region), or ROOM,
  * to be decoded whole (a fallback).
  */
-static int gz_split_finish(dng_scan *s, const std::vector<dng_scan::GzFile> &q,
+static int gz_split_finish(dng_scan *s, const std::vector<dng_scan::CzFile> &q,
     const std::vector<size_t> &out_off, std::vector<GzSplitFile> &sf,
     std::vector<GzChunk> &ck, std::vector<InfResult> &by_file,
     std::vector<const u8 *> &alt)
@@ -2250,41 +2267,23 @@ static int gz_split_finish(dng_scan *s, const std::vector<dng_scan::GzFile> &q,
 	return 0;
 }
 
-/* inflate and feed the queued gzip files, in the order they were fed */
-static int gz_flush(dng_scan *s)
+static int bz_batch(dng_scan *s, const std::vector<dng_scan::CzFile> &q,
+    const std::vector<size_t> &in_off);
+
+/* inflate and feed a batch of gzip files, whose compressed bytes are in
+ * d_cz_in at in_off, in the order they were fed */
+static int gz_batch(dng_scan *s, const std::vector<dng_scan::CzFile> &q,
+    const std::vector<size_t> &in_off)
 {
-	if (s->gz_queue.empty())
-		return s->err_code;
-	std::vector<dng_scan::GzFile> q;
-	q.swap(s->gz_queue);
-	s->gz_queued_in = s->gz_queued_out = 0;
-	if (s->err_code)
-		return s->err_code;
 	const size_t n = q.size();
-	std::vector<size_t> in_off(n), out_off(n);
-	size_t tin = 0, tout = 0;
+	std::vector<size_t> out_off(n);
+	size_t tout = 0;
 	for (size_t i = 0; i < n; i++) {
-		in_off[i] = tin;
-		tin += round16(q[i].size);
 		out_off[i] = tout;
 		tout += q[i].hint;
 	}
-	if (gz_room(s, &s->d_gz_in, &s->gz_in_cap, tin) ||
-	    gz_room(s, &s->d_gz_out, &s->gz_out_cap, tout))
+	if (gz_room(s, &s->d_gz_out, &s->gz_out_cap, tout))
 		return s->err_code;
-	/* compressed bytes through the file reader (direct_read.h's policy) */
-	for (size_t i = 0; i < n; i++) {
-		const char *path = q[i].path.c_str();
-		int fd = open(path, O_RDONLY);
-		if (fd < 0)
-			return s->fail(DNG_EIO, std::string("open ") + path +
-			    ": " + strerror(errno));
-		const int rc = feed_file_parallel(s, fd, 0, q[i].size, path, true,
-		    s->d_gz_in + in_off[i]);
-		close(fd);
-		if (rc)
-			return rc;
-	}
 	/* large files of a batch of few: split (inflate_policy.h) */
 	std::vector<uint64_t> sizes(n);
 	for (size_t i = 0; i < n; i++)
@@ -2316,7 +2315,7 @@ static int gz_flush(dng_scan *s)
 		std::vector<InfResult> res(files.size());
 		for (size_t k = 0; k < files.size(); k++) {
 			const u32 i = files[k];
-			jobs[k] = { s->d_gz_in + in_off[i], q[i].size,
+			jobs[k] = { s->d_cz_in + in_off[i], q[i].size,
 			    s->d_gz_out + out_off[i], q[i].hint };
 		}
 		if (gz_launch(s, jobs.data(), (u32)files.size(), res.data()))
@@ -2377,7 +2376,7 @@ static int gz_flush(dng_scan *s)
 				    (uint64_t)1 << 20);
 				if (gz_room(s, &s->d_gz_big, &s->gz_big_cap, cap))
 					return s->err_code;
-				const InfJob j = { s->d_gz_in + in_off[i],
+				const InfJob j = { s->d_cz_in + in_off[i],
 				    q[i].size, s->d_gz_big, cap };
 				if (gz_launch(s, &j, 1, &r))
 					return s->err_code;
@@ -2403,6 +2402,399 @@ static int gz_flush(dng_scan *s)
 		if (feed_device(s, src, len))
 			return s->err_code;
 	}
+	return 0;
+}
+
+/* read the queued compressed files to the device and decode and feed them,
+ * in the order they were fed */
+static int cz_flush(dng_scan *s)
+{
+	if (s->cz_queue.empty())
+		return s->err_code;
+	std::vector<dng_scan::CzFile> q;
+	q.swap(s->cz_queue);
+	s->cz_queued_in = s->cz_queued_out = 0;
+	if (s->err_code)
+		return s->err_code;
+	const size_t n = q.size();
+	std::vector<size_t> in_off(n);
+	size_t tin = 0;
+	for (size_t i = 0; i < n; i++) {
+		in_off[i] = tin;
+		tin += round16(q[i].size);
+	}
+	if (gz_room(s, &s->d_cz_in, &s->cz_in_cap, tin))
+		return s->err_code;
+	/* compressed bytes through the file reader (direct_read.h's policy) */
+	for (size_t i = 0; i < n; i++) {
+		const char *path = q[i].path.c_str();
+		int fd = open(path, O_RDONLY);
+		if (fd < 0)
+			return s->fail(DNG_EIO, std::string("open ") + path +
+			    ": " + strerror(errno));
+		const int rc = feed_file_parallel(s, fd, 0, q[i].size, path, true,
+		    s->d_cz_in + in_off[i]);
+		close(fd);
+		if (rc)
+			return rc;
+	}
+	return s->cz_bzip2 ? bz_batch(s, q, in_off) : gz_batch(s, q, in_off);
+}
+
+/* ---- bzip2 files (dng_scan_feed_bzip2) -------------------------------------
+ *
+ * A batch (the queue's limits: 256 files, 512 MiB compressed) is decoded by
+ * the stages of bunzip.cuh.  bz_find_kernel finds every candidate magic of
+ * every file; after that wait the host sorts them per file and cuts the block
+ * candidates into waves (bunzip_policy.h).  Per wave: bz_decode_kernel
+ * decodes every candidate (one wait), the host advances each file's chain
+ * through them, bz_ibwt_kernel inverts the chained blocks and sizes their
+ * output (one wait), and bz_emit_kernel writes each group of blocks back to
+ * back, files in feed order, with their CRCs (one wait per group).  A group
+ * is fed as one device buffer once its CRCs hold.  Every buffer is written on
+ * the scan's stream, after the scan kernels that read it earlier.
+ */
+struct BzStage {
+	cudaEvent_t e0, e1;
+};
+
+static BzStage bz_stage_start(dng_scan *s)
+{
+	BzStage t = { get_event(s), get_event(s) };
+	cudaEventRecord(t.e0, s->stream);
+	return t;
+}
+
+/* the stage's kernels are launched: count them, close the timer */
+static void bz_stage_stop(dng_scan *s, BzStage &t, uint32_t launches)
+{
+	cudaEventRecord(t.e1, s->stream);
+	s->bz_launches += launches;
+	s->aux_launches += launches;
+}
+
+/* once the stream is idle (or failed): its time into bunzip_ms */
+static void bz_stage_read(dng_scan *s, BzStage &t, int stage)
+{
+	float ms = 0;
+	if (cudaEventElapsedTime(&ms, t.e0, t.e1) == cudaSuccess) {
+		s->bz_ms += ms;
+		s->bz_stage_ms[stage] += ms;
+	}
+	s->ev_pool.push_back(t.e0);
+	s->ev_pool.push_back(t.e1);
+}
+
+static int bz_damage(dng_scan *s, const std::string &path, uint32_t kind,
+    uint64_t bit)
+{
+	const std::string what = kind == BE_TRAILING ?
+	    std::string(bunzip_error_name(kind)) :
+	    std::string("corrupt bzip2 data: ") + bunzip_error_name(kind);
+	return s->fail(DNG_EIO, path + ": " + what + " (compressed byte " +
+	    std::to_string(bit / 8) + ")");
+}
+
+static size_t bz_align(size_t n)
+{
+	return (n + 255) & ~(size_t)255;
+}
+
+/* every candidate magic of the batch, sorted by file and bit, and each
+ * file's one past its last nonzero byte */
+static int bz_find(dng_scan *s, const std::vector<dng_scan::CzFile> &q,
+    const std::vector<size_t> &in_off, std::vector<BzCand> &cand,
+    std::vector<unsigned long long> &nz)
+{
+	const size_t n = q.size();
+	uint64_t tin = 0, maxlen = 0;
+	std::vector<BzFile> files(n);
+	for (size_t i = 0; i < n; i++) {
+		files[i] = { s->d_cz_in + in_off[i], q[i].size };
+		tin += q[i].size;
+		maxlen = std::max<uint64_t>(maxlen, q[i].size);
+	}
+	const size_t o_nz = bz_align(n * sizeof (BzFile));
+	const size_t o_cnt = o_nz + bz_align(n * 8);
+	const size_t o_cand = o_cnt + 256;
+	size_t cap = tin / 512 + 4096;
+	uint32_t count = 0;
+	nz.assign(n, 0);
+	for (;;) {
+		if (gz_room(s, &s->d_bz_find, &s->bz_find_cap, o_cand +
+		    cap * sizeof (BzCand)))
+			return s->err_code;
+		CK(s, cudaMemcpyAsync(s->d_bz_find, files.data(),
+		    n * sizeof (BzFile), cudaMemcpyHostToDevice, s->stream));
+		CK(s, cudaMemsetAsync(s->d_bz_find + o_nz, 0, o_cand - o_nz,
+		    s->stream));
+		const uint64_t per = 256 * 16;	/* bytes per CTA and sweep */
+		const dim3 grid((u32)std::min<uint64_t>(std::max<uint64_t>(
+		    (maxlen + per - 1) / per, 1), 65535), (u32)n);
+		BzStage t = bz_stage_start(s);
+		bz_find_kernel<<<grid, 256, 0, s->stream>>>(
+		    (const BzFile *)s->d_bz_find,
+		    (BzCand *)(s->d_bz_find + o_cand), (u32)cap,
+		    (u32 *)(s->d_bz_find + o_cnt),
+		    (unsigned long long *)(s->d_bz_find + o_nz));
+		cudaError_t e = cudaGetLastError();
+		bz_stage_stop(s, t, 1);
+		if (e == cudaSuccess)
+			e = cudaMemcpyAsync(nz.data(), s->d_bz_find + o_nz, n * 8,
+			    cudaMemcpyDeviceToHost, s->stream);
+		if (e == cudaSuccess)
+			e = cudaMemcpyAsync(&count, s->d_bz_find + o_cnt, 4,
+			    cudaMemcpyDeviceToHost, s->stream);
+		if (e == cudaSuccess)
+			e = cudaStreamSynchronize(s->stream);
+		bz_stage_read(s, t, 0);
+		if (s->cuda(e, "bz_find_kernel"))
+			return s->err_code;
+		if (count <= cap)
+			break;
+		cap = count;	/* more candidates than room: find again */
+	}
+	cand.resize(count);
+	if (count) {
+		CK(s, cudaMemcpyAsync(cand.data(), s->d_bz_find + o_cand,
+		    count * sizeof (BzCand), cudaMemcpyDeviceToHost, s->stream));
+		CK(s, cudaStreamSynchronize(s->stream));
+	}
+	std::sort(cand.begin(), cand.end(), [](const BzCand &a,
+	    const BzCand &b) {
+		return a.file != b.file ? a.file < b.file : a.bit < b.bit;
+	});
+	return 0;
+}
+
+/* decode, chain, invert and emit a batch of bzip2 files (above) */
+static int bz_batch(dng_scan *s, const std::vector<dng_scan::CzFile> &q,
+    const std::vector<size_t> &in_off)
+{
+	const size_t n = q.size();
+	std::vector<BzCand> cand;
+	std::vector<unsigned long long> nz;
+	if (bz_find(s, q, in_off, cand, nz))
+		return s->err_code;
+	/* each file's candidates, and the block candidates in order */
+	std::vector<u32> fbeg(n + 1, 0), bidx, which(cand.size(), ~0u);
+	for (const BzCand &c : cand)
+		fbeg[c.file + 1]++;
+	for (size_t i = 0; i < n; i++)
+		fbeg[i + 1] += fbeg[i];
+	for (u32 i = 0; i < cand.size(); i++)
+		if (cand[i].kind == BZ_CAND_BLOCK) {
+			which[i] = (u32)bidx.size();
+			bidx.push_back(i);
+		}
+	std::vector<size_t> ends(bidx.size() + 1);
+	const size_t nw = bz_waves(bidx.size(), DNG_BZ_WAVE_BLOCKS,
+	    ends.data());
+	std::vector<BzChain> ch(n);
+	for (size_t i = 0; i < n; i++)
+		bz_chain_init(ch[i], q[i].size, nz[i], q[i].head);
+	std::vector<BzDecResult> res(bidx.size());
+	size_t f = 0;	/* the first file whose chain is not done */
+	for (size_t w = 0, lo = 0;; w++) {
+		const size_t hi = w < nw ? ends[w] : lo, wn = hi - lo;
+		size_t o = 0;
+		auto at = [&](size_t bytes) {
+			const size_t r = o;
+			o += bz_align(bytes);
+			return r;
+		};
+		const size_t o_dj = at(wn * sizeof (BzDecJob));
+		const size_t o_dr = at(wn * sizeof (BzDecResult));
+		const size_t o_hist = at(wn * 256 * 4), o_next = at(16);
+		const size_t o_bj = at(wn * sizeof (BzBwtJob));
+		const size_t o_br = at(wn * sizeof (BzBwtResult));
+		const size_t o_ck = at(wn * BZ_CHUNKS * 8);
+		const size_t o_ej = at(wn * sizeof (BzEmitJob));
+		const size_t o_crc = at(wn * 4);
+		u8 *rec = nullptr;
+		if (wn) {
+			/* decode the wave's candidates, one warp each */
+			if (gz_room(s, &s->d_bz_rec, &s->bz_rec_cap, o) ||
+			    gz_room(s, &s->d_bz_slot, &s->bz_slot_cap,
+			    wn * (size_t)BZ_SLOT))
+				return s->err_code;
+			rec = s->d_bz_rec;
+			std::vector<BzDecJob> dj(wn);
+			for (size_t k = 0; k < wn; k++) {
+				const BzCand &c = cand[bidx[lo + k]];
+				dj[k] = { s->d_cz_in + in_off[c.file],
+				    q[c.file].size, c.bit,
+				    s->d_bz_slot + k * (size_t)BZ_SLOT,
+				    (uint32_t *)(rec + o_hist) + k * 256 };
+			}
+			CK(s, cudaMemcpyAsync(rec + o_dj, dj.data(),
+			    wn * sizeof (BzDecJob), cudaMemcpyHostToDevice,
+			    s->stream));
+			CK(s, cudaMemsetAsync(rec + o_next, 0, 16, s->stream));
+			const u32 grid = (u32)std::min<size_t>((wn + BZ_DEC_WARPS -
+			    1) / BZ_DEC_WARPS, (size_t)s->sm_count * 8);
+			BzStage t = bz_stage_start(s);
+			bz_decode_kernel<<<grid, 32 * BZ_DEC_WARPS, 0,
+			    s->stream>>>((const BzDecJob *)(rec + o_dj),
+			    (BzDecResult *)(rec + o_dr), (u32)wn,
+			    (u32 *)(rec + o_next));
+			cudaError_t e = cudaGetLastError();
+			bz_stage_stop(s, t, 1);
+			if (e == cudaSuccess)
+				e = cudaMemcpyAsync(res.data() + lo, rec + o_dr,
+				    wn * sizeof (BzDecResult),
+				    cudaMemcpyDeviceToHost, s->stream);
+			if (e == cudaSuccess)
+				e = cudaStreamSynchronize(s->stream);
+			bz_stage_read(s, t, 1);
+			if (s->cuda(e, "bz_decode_kernel"))
+				return s->err_code;
+		}
+		/* chain every file the decodes so far reach, in feed order; a
+		 * damaged file stops it, and fails the scan once the blocks
+		 * before the damage have passed their CRCs */
+		std::vector<u32> took;
+		bool early = false;
+		size_t damaged = n;
+		for (; f < n; f++) {
+			BzChain &c = ch[f];
+			const u32 b0 = fbeg[f];
+			bz_chain_run(c, cand.data() + b0, fbeg[f + 1] - b0,
+			    [&](u32 i) -> const BzDecResult * {
+				const size_t k = which[b0 + i];
+				return k < hi ? &res[k] : nullptr;
+			    }, [&](u32 i) {
+				early |= which[b0 + i] < lo;
+				took.push_back(which[b0 + i]);
+			    });
+			if (c.kind) {
+				damaged = f;
+				break;
+			}
+			if (early)
+				return s->fail(DNG_EIO, q[f].path + ": bzip2 "
+				    "chain went back to an earlier wave");
+			if (!c.done)
+				break;
+		}
+		s->bz_false_starts += wn - took.size();
+		const size_t m = took.size();
+		if (m) {
+			/* invert the chained blocks, one CTA each */
+			std::vector<size_t> tt_off(m);
+			size_t tsum = 0;
+			for (size_t k = 0; k < m; k++) {
+				tt_off[k] = tsum;
+				tsum += round16((size_t)res[took[k]].nblock * 4);
+			}
+			if (gz_room(s, &s->d_bz_tt, &s->bz_tt_cap, tsum))
+				return s->err_code;
+			std::vector<BzBwtJob> bj(m);
+			for (size_t k = 0; k < m; k++) {
+				const size_t c = took[k] - lo;
+				const BzDecResult &r = res[took[k]];
+				bj[k] = { s->d_bz_slot + c * (size_t)BZ_SLOT,
+				    (uint32_t *)(s->d_bz_tt + tt_off[k]),
+				    (const uint32_t *)(rec + o_hist) + c * 256,
+				    (uint32_t *)(rec + o_ck) + k * BZ_CHUNKS * 2,
+				    r.nblock, r.orig, r.rand, 0 };
+			}
+			CK(s, cudaMemcpyAsync(rec + o_bj, bj.data(),
+			    m * sizeof (BzBwtJob), cudaMemcpyHostToDevice,
+			    s->stream));
+			std::vector<BzBwtResult> br(m);
+			BzStage t = bz_stage_start(s);
+			bz_ibwt_kernel<<<(u32)m, BZ_THREADS, 0, s->stream>>>(
+			    (const BzBwtJob *)(rec + o_bj),
+			    (BzBwtResult *)(rec + o_br));
+			cudaError_t e = cudaGetLastError();
+			bz_stage_stop(s, t, 1);
+			if (e == cudaSuccess)
+				e = cudaMemcpyAsync(br.data(), rec + o_br,
+				    m * sizeof (BzBwtResult),
+				    cudaMemcpyDeviceToHost, s->stream);
+			if (e == cudaSuccess)
+				e = cudaStreamSynchronize(s->stream);
+			bz_stage_read(s, t, 2);
+			if (s->cuda(e, "bz_ibwt_kernel"))
+				return s->err_code;
+			std::vector<uint64_t> lens(m);
+			for (size_t k = 0; k < m; k++) {
+				const BzCand &c = cand[bidx[took[k]]];
+				if (!br[k].ok)	/* a run without its count */
+					return bz_damage(s, q[c.file].path,
+					    BE_OVERFLOW, c.bit);
+				lens[k] = br[k].out_len;
+			}
+			/* emit in groups, each fed once its CRCs hold */
+			std::vector<size_t> gend(m);
+			const size_t ng = bz_emit_groups(lens.data(), m,
+			    DNG_BZ_EMIT_OUT, gend.data());
+			for (size_t g = 0, g0 = 0; g < ng; g0 = gend[g++]) {
+				const size_t g1 = gend[g];
+				uint64_t sum = 0;
+				std::vector<BzEmitJob> ej(g1 - g0);
+				for (size_t k = g0; k < g1; k++)
+					sum += lens[k];
+				if (gz_room(s, &s->d_bz_out, &s->bz_out_cap, sum))
+					return s->err_code;
+				uint64_t off = 0;
+				for (size_t k = g0; k < g1; k++) {
+					ej[k - g0] = { bj[k].slot, bj[k].chunks,
+					    s->d_bz_out + off, bj[k].n, 0 };
+					off += lens[k];
+				}
+				CK(s, cudaMemcpyAsync(rec + o_ej, ej.data(),
+				    ej.size() * sizeof (BzEmitJob),
+				    cudaMemcpyHostToDevice, s->stream));
+				std::vector<uint32_t> crc(g1 - g0);
+				BzStage te = bz_stage_start(s);
+				bz_emit_kernel<<<(u32)(g1 - g0), BZ_THREADS, 0,
+				    s->stream>>>((const BzEmitJob *)(rec + o_ej),
+				    (uint32_t *)(rec + o_crc));
+				e = cudaGetLastError();
+				bz_stage_stop(s, te, 1);
+				if (e == cudaSuccess)
+					e = cudaMemcpyAsync(crc.data(), rec + o_crc,
+					    crc.size() * 4,
+					    cudaMemcpyDeviceToHost, s->stream);
+				if (e == cudaSuccess)
+					e = cudaStreamSynchronize(s->stream);
+				bz_stage_read(s, te, 3);
+				if (s->cuda(e, "bz_emit_kernel"))
+					return s->err_code;
+				for (size_t k = g0; k < g1; k++)
+					if (crc[k - g0] != res[took[k]].crc) {
+						const BzCand &c =
+						    cand[bidx[took[k]]];
+						return bz_damage(s,
+						    q[c.file].path,
+						    BE_BLOCK_CRC, c.bit);
+					}
+				s->bz_out_bytes += sum;
+				if (feed_device(s, s->d_bz_out, sum))
+					return s->err_code;
+			}
+		}
+		if (damaged < n)
+			return bz_damage(s, q[damaged].path, ch[damaged].kind,
+			    ch[damaged].err_bit);
+		lo = hi;
+		if (f == n) {
+			/* candidates past every chain's end: never decoded */
+			s->bz_false_starts += bidx.size() - hi;
+			break;
+		}
+		if (w >= nw)
+			return s->fail(DNG_EIO, q[f].path + ": bzip2 chain "
+			    "stopped before its end");
+	}
+	for (size_t i = 0; i < n; i++) {
+		s->bz_in_bytes += q[i].size;
+		s->bz_streams += ch[i].streams;
+		s->bz_blocks += ch[i].blocks;
+	}
+	s->bz_files += n;
 	return 0;
 }
 
@@ -2439,13 +2831,15 @@ int dng_scan_feed_gzip(dng_scan *s, const char *path)
 	}
 	const size_t size = (size_t)st.st_size;
 	const uint64_t hint = trailer ? inflate_hint(tail, size) : 0;
-	if (!s->gz_queue.empty() && (s->gz_queue.size() >= GZ_BATCH_FILES ||
-	    s->gz_queued_in + round16(size) > GZ_BATCH_IN ||
-	    s->gz_queued_out + hint > GZ_BATCH_OUT) && gz_flush(s))
+	if (!s->cz_queue.empty() && (s->cz_bzip2 ||
+	    s->cz_queue.size() >= GZ_BATCH_FILES ||
+	    s->cz_queued_in + round16(size) > GZ_BATCH_IN ||
+	    s->cz_queued_out + hint > GZ_BATCH_OUT) && cz_flush(s))
 		return s->err_code;
-	s->gz_queue.push_back({ path, size, hint });
-	s->gz_queued_in += round16(size);
-	s->gz_queued_out += hint;
+	s->cz_bzip2 = false;
+	s->cz_queue.push_back({ path, size, hint, 0 });
+	s->cz_queued_in += round16(size);
+	s->cz_queued_out += hint;
 	return DNG_OK;
 }
 
@@ -2489,6 +2883,84 @@ int dng_scan_gzip_split_stats(dng_scan *s, uint64_t *split_files,
 	return DNG_OK;
 }
 
+int dng_scan_feed_bzip2(dng_scan *s, const char *path)
+{
+	if (!s || !path)
+		return DNG_EINVAL;
+	if (s->multi)
+		return refuse_multi(s, "dng_scan_feed_bzip2");
+	if (s->err_code)
+		return s->err_code;
+	if (s->finished)
+		return s->fail(DNG_EINVAL, "scan already finished");
+	cudaSetDevice(s->device);
+	int fd = open(path, O_RDONLY);
+	if (fd < 0)
+		return s->fail(DNG_EIO, std::string("open ") + path + ": " +
+		    strerror(errno));
+	struct stat st;
+	u8 h[4] = {};
+	const bool reg = fstat(fd, &st) == 0 && S_ISREG(st.st_mode);
+	const bool got = reg && st.st_size >= 4 && pread(fd, h, 4, 0) == 4;
+	close(fd);
+	const uint32_t head = (uint32_t)h[0] << 24 | (uint32_t)h[1] << 16 |
+	    (uint32_t)h[2] << 8 | h[3];
+	if (!got || !bz_level_ok(head)) {
+		/* refused, not failed: the scan goes on */
+		if (!s->err_code)
+			s->err = std::string(path) + (reg ? ": not a bzip2 file "
+			    "(it does not start with BZh and a level 1-9)" :
+			    ": not a regular file");
+		return DNG_EINVAL;
+	}
+	const size_t size = (size_t)st.st_size;
+	if (!s->cz_queue.empty() && (!s->cz_bzip2 ||
+	    s->cz_queue.size() >= GZ_BATCH_FILES ||
+	    s->cz_queued_in + round16(size) > GZ_BATCH_IN) && cz_flush(s))
+		return s->err_code;
+	s->cz_bzip2 = true;
+	s->cz_queue.push_back({ path, size, 0, head });
+	s->cz_queued_in += round16(size);
+	return DNG_OK;
+}
+
+int dng_scan_bzip2_stats(dng_scan *s, uint64_t *files, uint64_t *streams,
+    uint64_t *blocks, uint64_t *false_starts, uint64_t *compressed_bytes,
+    uint64_t *decompressed_bytes, uint64_t *launches, double *bunzip_ms)
+{
+	if (!s)
+		return DNG_EINVAL;
+	if (files)
+		*files = s->bz_files;
+	if (streams)
+		*streams = s->bz_streams;
+	if (blocks)
+		*blocks = s->bz_blocks;
+	if (false_starts)
+		*false_starts = s->bz_false_starts;
+	if (compressed_bytes)
+		*compressed_bytes = s->bz_in_bytes;
+	if (decompressed_bytes)
+		*decompressed_bytes = s->bz_out_bytes;
+	if (launches)
+		*launches = s->bz_launches;
+	if (bunzip_ms)
+		*bunzip_ms = s->bz_ms;
+	return DNG_OK;
+}
+
+int dng_scan_bzip2_stage_ms(dng_scan *s, double *find_ms, double *decode_ms,
+    double *invert_ms, double *emit_ms)
+{
+	if (!s)
+		return DNG_EINVAL;
+	double *const out[4] = { find_ms, decode_ms, invert_ms, emit_ms };
+	for (int i = 0; i < 4; i++)
+		if (out[i])
+			*out[i] = s->bz_stage_ms[i];
+	return DNG_OK;
+}
+
 int dng_scan_sync(dng_scan *s)
 {
 	if (!s)
@@ -2496,7 +2968,7 @@ int dng_scan_sync(dng_scan *s)
 	if (s->multi)	/* (its shards run only inside dng_scan_finish) */
 		return s->err_code;
 	cudaSetDevice(s->device);
-	gz_flush(s);
+	cz_flush(s);
 	CK(s, cudaStreamSynchronize(s->copy_stream));
 	CK(s, cudaStreamSynchronize(s->stream));
 	drain_events(s);
@@ -2609,7 +3081,7 @@ int dng_scan_finish(dng_scan *s, dng_result **out)
 	if (s->multi)
 		return finish_multi(s, out);
 	cudaSetDevice(s->device);
-	if (gz_flush(s) || flush_tail(s))
+	if (cz_flush(s) || flush_tail(s))
 		return s->err_code;
 	if (dng_scan_sync(s))
 		return s->err_code;
@@ -2931,7 +3403,7 @@ void dng_scan_destroy(dng_scan *s)
 	cached_free(s->d_nl);
 	cached_free(s->d_carry);
 	cached_free(s->d_side);
-	cached_free(s->d_gz_in);
+	cached_free(s->d_cz_in);
 	cached_free(s->d_gz_out);
 	cached_free(s->d_gz_big);
 	cached_free(s->d_gz_join);
@@ -2941,6 +3413,11 @@ void dng_scan_destroy(dng_scan *s)
 	cached_free(s->d_gz_sym);
 	cached_free(s->d_gz_sout);
 	cached_free(s->d_gz_check);
+	cached_free(s->d_bz_find);
+	cached_free(s->d_bz_slot);
+	cached_free(s->d_bz_tt);
+	cached_free(s->d_bz_rec);
+	cached_free(s->d_bz_out);
 	if (s->own_stream)
 		cudaStreamDestroy(s->own_stream);
 	if (s->copy_stream)

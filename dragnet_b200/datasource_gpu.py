@@ -94,13 +94,21 @@ def stage_counters(plan, c, npoints):
 
 
 GZIP_MAGIC = b'\x1f\x8b\x08'
-COMPRESSIONS = (None, 'none', 'gzip')
+COMPRESSIONS = (None, 'none', 'gzip', 'bzip2')
 
 
 def is_gzip(path):
     """Whether the file starts as a gzip member of DEFLATE data does."""
     with open(path, 'rb') as f:
         return f.read(3) == GZIP_MAGIC
+
+
+def is_bzip2(path):
+    """Whether the file starts as a bzip2 stream does: BZh and a level
+    digit 1-9."""
+    with open(path, 'rb') as f:
+        head = f.read(4)
+    return len(head) == 4 and head[:3] == b'BZh' and 0x31 <= head[3] <= 0x39
 
 
 def run_plan(plan, files=(), chunks=None, device=0, device_buffers=None,
@@ -110,13 +118,16 @@ def run_plan(plan, files=(), chunks=None, device=0, device_buffers=None,
     than one device index -> one scan over all of them, the files cut into a
     byte range per device (files only); its stats are per shard.
     compression 'gzip': files that start with 1f 8b 08 are inflated on the
-    device (dng_scan_feed_gzip), others read as they are; one device only."""
+    device (dng_scan_feed_gzip), others read as they are; 'bzip2': files
+    that start with BZh and a level 1-9 are decoded on the device
+    (dng_scan_feed_bzip2), others read as they are; one device only."""
     import json
     multi = devices is not None and len(devices) > 1
     gzip = compression == 'gzip'
-    if gzip and multi:
-        raise DsError('compression "gzip" is not supported on a scan over '
-                      'several devices')
+    bzip2 = compression == 'bzip2'
+    if (gzip or bzip2) and multi:
+        raise DsError('compression "%s" is not supported on a scan over '
+                      'several devices' % compression)
     p = native.Plan(json.dumps(plan, separators=(',', ':')))
     if devices and not multi:
         device = devices[0]
@@ -128,6 +139,8 @@ def run_plan(plan, files=(), chunks=None, device=0, device_buffers=None,
         for f in files:
             if gzip and is_gzip(f):
                 s.feed_gzip(f)
+            elif bzip2 and is_bzip2(f):
+                s.feed_bzip2(f)
             else:
                 s.feed_file(f)
         for c in (chunks or ()):
@@ -150,6 +163,8 @@ def run_plan(plan, files=(), chunks=None, device=0, device_buffers=None,
             if gzip:
                 stats.update(s.gzip_stats())
                 stats.update(s.gzip_split_stats())
+            if bzip2:
+                stats.update(s.bzip2_stats())
         pts = []
         if 'metrics' in plan:
             # fan-out: points are tagged like the reference tags them
@@ -193,7 +208,8 @@ class DatasourceGpu(object):
         # a list of device indices, or "all": one scan over all of them
         # (files cut by bytes, tallies merged exactly), else ds_device alone
         self.ds_devices = dsconfig.get('devices')
-        # "gzip": gzip files among the input are inflated on the device
+        # "gzip" / "bzip2": files of that format among the input are
+        # decoded on the device
         self.ds_compression = bc.get('compression')
         if self.ds_compression == 'none':
             self.ds_compression = None
@@ -212,9 +228,10 @@ class DatasourceGpu(object):
 
     def _run(self, plan, files):
         devices = self._devices()
-        if self.ds_compression == 'gzip' and devices and len(devices) > 1:
-            return DsError('compression "gzip" is not supported on a scan '
-                           'over several devices')
+        if self.ds_compression in ('gzip', 'bzip2') and devices and \
+                len(devices) > 1:
+            return DsError('compression "%s" is not supported on a scan '
+                           'over several devices' % self.ds_compression)
         return run_plan(plan, files=files, device=self.ds_device,
                         devices=devices, compression=self.ds_compression)
 

@@ -68,6 +68,7 @@ _SIGS = [
     ('dng_scan_feed_device', ctypes.c_int, [_P, _P, ctypes.c_size_t]),
     ('dng_scan_feed_file', ctypes.c_int, [_P, ctypes.c_char_p]),
     ('dng_scan_feed_gzip', ctypes.c_int, [_P, ctypes.c_char_p]),
+    ('dng_scan_feed_bzip2', ctypes.c_int, [_P, ctypes.c_char_p]),
     ('dng_scan_sync', ctypes.c_int, [_P]),
     ('dng_scan_finish', ctypes.c_int, [_P, ctypes.POINTER(_P)]),
     ('dng_scan_counters', ctypes.c_int, [_P, ctypes.POINTER(DngCounters)]),
@@ -100,6 +101,11 @@ _SIGS = [
      [ctypes.POINTER(ctypes.c_double)]),
     ('dng_scan_gzip_split_stats', ctypes.c_int,
      [_P] + [ctypes.POINTER(ctypes.c_uint64)] * 5),
+    ('dng_scan_bzip2_stats', ctypes.c_int,
+     [_P] + [ctypes.POINTER(ctypes.c_uint64)] * 7 +
+     [ctypes.POINTER(ctypes.c_double)]),
+    ('dng_scan_bzip2_stage_ms', ctypes.c_int,
+     [_P] + [ctypes.POINTER(ctypes.c_double)] * 4),
     ('dng_scan_launch_count', ctypes.c_uint64, [_P]),
     ('dng_pinned_alloc', _P, [ctypes.c_size_t]),
     ('dng_pinned_free', None, [_P]),
@@ -180,6 +186,10 @@ GZIP_STATS = ['gzip_files', 'gzip_members', 'gzip_compressed_bytes',
               'gzip_inflated_bytes', 'inflate_launches', 'inflate_ms']
 GZIP_SPLIT_STATS = ['gzip_split_files', 'gzip_chunks', 'gzip_false_starts',
                     'gzip_fallbacks', 'gzip_split_launches']
+BZIP2_STATS = ['bzip2_files', 'bzip2_streams', 'bzip2_blocks',
+               'bzip2_false_starts', 'bzip2_compressed_bytes',
+               'bzip2_decompressed_bytes', 'bunzip_launches', 'bunzip_ms']
+BZIP2_STAGES = ['find', 'decode', 'invert', 'emit']
 
 
 def set_jit_cache_dir(path):
@@ -418,6 +428,24 @@ class _ScanStats(object):
             self.handle, *[ctypes.byref(x) for x in v]), self.handle)
         return dict(zip(GZIP_SPLIT_STATS, (int(x.value) for x in v)))
 
+    def bzip2_stats(self):
+        """What dng_scan_feed_bzip2 decoded: files, streams, blocks, block
+        candidates the chain did not land on, compressed and decompressed
+        bytes, bzip2 kernel launches and milliseconds."""
+        v = [ctypes.c_uint64() for _ in range(7)]
+        ms = ctypes.c_double()
+        _check(lib().dng_scan_bzip2_stats(self.handle,
+                                          *[ctypes.byref(x) for x in v],
+                                          ctypes.byref(ms)), self.handle)
+        return dict(zip(BZIP2_STATS, [int(x.value) for x in v] + [ms.value]))
+
+    def bzip2_stage_ms(self):
+        """bunzip_ms by stage: find, decode, invert, emit."""
+        v = [ctypes.c_double() for _ in BZIP2_STAGES]
+        _check(lib().dng_scan_bzip2_stage_ms(
+            self.handle, *[ctypes.byref(x) for x in v]), self.handle)
+        return dict(zip(BZIP2_STAGES, (x.value for x in v)))
+
 
 class Scan(_ScanStats):
     def __init__(self, plan, device=0, devices=None):
@@ -463,6 +491,13 @@ class Scan(_ScanStats):
         """A gzip file, inflated on the device; queued, and processed no
         later than the next feed, sync or finish."""
         _check(lib().dng_scan_feed_gzip(self.handle, os.fsencode(path)),
+               self.handle)
+
+    def feed_bzip2(self, path):
+        """A bzip2 file, decoded on the device with its blocks in
+        parallel; queued with gzip files, and processed no later than the
+        next feed of another kind, sync or finish."""
+        _check(lib().dng_scan_feed_bzip2(self.handle, os.fsencode(path)),
                self.handle)
 
     def sync(self):

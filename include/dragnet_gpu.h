@@ -206,6 +206,36 @@ int dng_scan_gzip_split_stats(dng_scan *scan, uint64_t *split_files,
     uint64_t *chunks, uint64_t *false_starts, uint64_t *fallbacks,
     uint64_t *launches);
 
+/*
+ * dng_scan_feed_bzip2: a bzip2 file (one or more complete streams, levels
+ *   BZh1-BZh9 mixed, randomised blocks included, optionally followed by zero
+ *   bytes), decoded on the device with all its blocks in parallel.  Its
+ *   decompressed bytes join the scan's stream at this point, as for
+ *   dng_scan_feed_gzip.  A file that does not start with "BZh" and a digit
+ *   1-9 fails here with DNG_EINVAL.  It shares the gzip queue: a batch holds
+ *   files of one format, and a feed of another kind processes the queue
+ *   first.  Damage (bad stream or block header, bad selectors or code
+ *   lengths, an invalid code, a block overflow, a block or stream CRC
+ *   mismatch, truncation) fails the scan with DNG_EIO naming the file, the
+ *   damage and the compressed byte; so does anything after the last stream
+ *   that is not zero bytes, which Python's bz2.decompress would ignore.  A
+ *   scan over several devices refuses it (DNG_EINVAL).
+ */
+int dng_scan_feed_bzip2(dng_scan *scan, const char *path);
+/* Bzip2 files decoded so far, their streams and blocks, block candidates
+ * the chain of blocks did not land on (false starts), compressed and
+ * decompressed bytes, launches of the bzip2 kernels (also in
+ * dng_scan_launch_count) and their time (CUDA events).  Any pointer may be
+ * NULL. */
+int dng_scan_bzip2_stats(dng_scan *scan, uint64_t *files, uint64_t *streams,
+    uint64_t *blocks, uint64_t *false_starts, uint64_t *compressed_bytes,
+    uint64_t *decompressed_bytes, uint64_t *launches, double *bunzip_ms);
+/* bunzip_ms by stage: finding magics, decoding blocks, inverting them
+ * (inverse BWT and run lengths), emitting them (final run-length stage and
+ * CRCs). */
+int dng_scan_bzip2_stage_ms(dng_scan *scan, double *find_ms,
+    double *decode_ms, double *invert_ms, double *emit_ms);
+
 /* End of input: flushes the final unterminated line, then emits the points. */
 int dng_scan_finish(dng_scan *scan, dng_result **out);
 int dng_scan_counters(dng_scan *scan, dng_counters *out);

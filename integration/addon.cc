@@ -18,6 +18,7 @@
  *   scan.feed(buffer, cb)          dng_scan_feed      (bytes are consumed)
  *   scan.feedFile(path, cb)        dng_scan_feed_file
  *   scan.feedGzip(path, cb)        dng_scan_feed_gzip (inflated on the GPU)
+ *   scan.feedBzip2(path, cb)       dng_scan_feed_bzip2 (decoded on the GPU)
  *   scan.finish(cb)             -> cb(err, points, counters)
  *                                  points   = [{fields: {name: string|number},
  *                                              value: N}, ...]
@@ -89,7 +90,7 @@ struct Work {
 	napi_async_work work = nullptr;
 	napi_ref cb = nullptr, keep = nullptr;	/* callback; Buffer being fed */
 	ScanWrap *w = nullptr;
-	enum { FEED, FEED_FILE, FEED_GZIP, FINISH } op = FEED;
+	enum { FEED, FEED_FILE, FEED_GZIP, FEED_BZIP2, FINISH } op = FEED;
 	std::string path;
 	const void *buf = nullptr;
 	size_t len = 0;
@@ -110,6 +111,9 @@ void Exec(napi_env, void *d)
 		break;
 	case Work::FEED_GZIP:
 		k->rc = dng_scan_feed_gzip(k->w->scan, k->path.c_str());
+		break;
+	case Work::FEED_BZIP2:
+		k->rc = dng_scan_feed_bzip2(k->w->scan, k->path.c_str());
 		break;
 	case Work::FINISH:
 		k->rc = dng_scan_finish(k->w->scan, &k->res);
@@ -284,6 +288,25 @@ napi_value FeedGzip(napi_env env, napi_callback_info info)
 	return Queue(env, k, argv[1], "dragnet_gpu.feedGzip");
 }
 
+/* scan.feedBzip2(path, cb) */
+napi_value FeedBzip2(napi_env env, napi_callback_info info)
+{
+	size_t argc = 2;
+	napi_value argv[2];
+	ScanWrap *w = Unwrap(env, info, &argc, argv);
+	if (!w)
+		return nullptr;
+	if (argc < 2) {
+		Throw(env, "feedBzip2(path, callback)");
+		return nullptr;
+	}
+	Work *k = new Work();
+	k->w = w;
+	k->op = Work::FEED_BZIP2;
+	k->path = GetString(env, argv[0]);
+	return Queue(env, k, argv[1], "dragnet_gpu.feedBzip2");
+}
+
 /* scan.finish(cb) */
 napi_value Finish(napi_env env, napi_callback_info info)
 {
@@ -399,7 +422,8 @@ napi_value ScanOpen(napi_env env, napi_callback_info info)
 	napi_wrap(env, obj, w, Finalize, nullptr, nullptr);
 	const struct { const char *name; napi_callback fn; } methods[] = {
 	    { "feed", Feed }, { "feedFile", FeedFile },
-	    { "feedGzip", FeedGzip }, { "finish", Finish },
+	    { "feedGzip", FeedGzip },
+	    { "feedBzip2", FeedBzip2 }, { "finish", Finish },
 	    { "close", Close } };
 	for (const auto &m : methods) {
 		napi_create_function(env, m.name, NAPI_AUTO_LENGTH, m.fn, nullptr,

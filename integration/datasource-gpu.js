@@ -40,18 +40,19 @@ exports.createDatasource = function createDatasource(args)
 	if (typeof (args.dsconfig.ds_backend_config.path) != 'string')
 		return (new VError('expected datasource "path" to be a string'));
 	comp = args.dsconfig.ds_backend_config.compression;
-	if (comp !== undefined && comp !== 'none' && comp !== 'gzip')
+	if (comp !== undefined && comp !== 'none' && comp !== 'gzip' &&
+	    comp !== 'bzip2')
 		return (new VError('unsupported compression: "%s"', comp));
 	/*
-	 * "all" on a host with one GPU is a scan on that GPU and reads gzip
-	 * files, as in DatasourceGpu in Python; on several GPUs the scan over
-	 * all of them refuses feedGzip with DNG_EINVAL.
+	 * "all" on a host with one GPU is a scan on that GPU and reads
+	 * compressed files, as in DatasourceGpu in Python; on several GPUs the
+	 * scan over all of them refuses feedGzip and feedBzip2 with DNG_EINVAL.
 	 */
-	if (comp === 'gzip' &&
+	if ((comp === 'gzip' || comp === 'bzip2') &&
 	    Array.isArray(args.dsconfig.ds_backend_config.devices) &&
 	    args.dsconfig.ds_backend_config.devices.length > 1)
-		return (new VError('compression "gzip" is not supported on a ' +
-		    'scan over several devices'));
+		return (new VError('compression "%s" is not supported on a ' +
+		    'scan over several devices', comp));
 
 	/* (before the first scan is opened) */
 	if (args.jitCacheDir !== undefined && !jitCacheDirSet) {
@@ -85,20 +86,27 @@ function DatasourceGpu(args, fileds)
 		this.ds_device = args.dsconfig.ds_backend_config.devices;
 	/*
 	 * "compression": "gzip": files that start with 1f 8b 08 (rotated logs)
-	 * are inflated on the GPU (dng_scan_feed_gzip), any other file (the
-	 * live log beside them) is read as it is.
+	 * are inflated on the GPU (dng_scan_feed_gzip); "bzip2": files that
+	 * start with BZh and a level 1-9 are decoded on the GPU
+	 * (dng_scan_feed_bzip2).  Any other file (the live log beside them) is
+	 * read as it is.
 	 */
-	this.ds_gzip = args.dsconfig.ds_backend_config.compression === 'gzip';
+	this.ds_compression = args.dsconfig.ds_backend_config.compression;
+	if (this.ds_compression !== 'gzip' && this.ds_compression !== 'bzip2')
+		this.ds_compression = null;
 	this.ds_log = args.log;
 }
 
 /*
- * Feed one file to a scan: feedGzip() for a gzip file when the datasource
- * reads them, else feedFile().  Both are N-API async work items.
+ * Feed one file to a scan: feedGzip() or feedBzip2() for a file of the
+ * datasource's compression, else feedFile().  All are N-API async work
+ * items.
  */
 DatasourceGpu.prototype.feedPath = function (scan, path, callback)
 {
-	if (!this.ds_gzip) {
+	var comp = this.ds_compression;
+
+	if (comp === null) {
 		scan.feedFile(path, callback);
 		return;
 	}
@@ -107,16 +115,20 @@ DatasourceGpu.prototype.feedPath = function (scan, path, callback)
 			callback(err);
 			return;
 		}
-		var head = Buffer.alloc(3);
-		mod_fs.read(fd, head, 0, 3, 0, function (rerr, n) {
+		var head = Buffer.alloc(4);
+		mod_fs.read(fd, head, 0, 4, 0, function (rerr, n) {
 			mod_fs.close(fd, function () {});
 			if (rerr) {
 				callback(rerr);
 				return;
 			}
-			if (n == 3 && head[0] == 0x1f && head[1] == 0x8b &&
-			    head[2] == 0x08)
+			if (comp === 'gzip' && n >= 3 && head[0] == 0x1f &&
+			    head[1] == 0x8b && head[2] == 0x08)
 				scan.feedGzip(path, callback);
+			else if (comp === 'bzip2' && n == 4 && head[0] == 0x42 &&
+			    head[1] == 0x5a && head[2] == 0x68 &&
+			    head[3] >= 0x31 && head[3] <= 0x39)
+				scan.feedBzip2(path, callback);
 			else
 				scan.feedFile(path, callback);
 		});
