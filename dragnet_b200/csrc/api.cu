@@ -1,5 +1,6 @@
 /*
- * api.cu: the C ABI of libdragnet_gpu.so (include/dragnet_gpu.h).
+ * api.cu: the C ABI of libdragnet_gpu.so (include/dragnet_gpu.h), but for
+ * compressed input (compressed.cu).
  *
  * Host-side plumbing only: device buffers, the H2D ring that keeps PCIe busy
  * while the previous chunk is being scanned, line carry between chunks
@@ -29,23 +30,18 @@
 #include "../../include/dragnet_gpu.h"
 #include "plan.h"
 #include "result.h"
+#include "scan.h"
 #include "scan_kernel.cuh"
 #include "fast_kernel.cuh"
 #include "jit.h"
 #include "jit_cache.h"
 #include "gen.cuh"
 #include "direct_read.h"
-#include "inflate.cuh"
-#include "inflate_policy.h"
-#include "inflate_split.cuh"
-#include "bunzip.cuh"
-#include "bunzip_policy.h"
 
 using namespace dng;
 
 namespace {
 
-const size_t RING_SLOTS = 3;
 const size_t CARRY_ROOM = (size_t)DNG_MAXREC + 4096;	/* room before a chunk */
 const size_t DNG_ARENA_MAX = (size_t)2 << 30;	/* largest DNG_ARENA_BYTES */
 
@@ -127,9 +123,6 @@ void cached_free(void *p)
 		cudaFree(p);
 }
 
-#define DEV_ALLOC(s, p, n) cached_alloc((s)->device, (void **)(p), (n))
-#define HOST_ALLOC(p, n) cached_alloc(-1, (void **)(p), (n))
-
 void set_err(char *err, size_t errlen, const char *fmt, const char *a = "")
 {
 	if (err && errlen)
@@ -138,7 +131,7 @@ void set_err(char *err, size_t errlen, const char *fmt, const char *a = "")
 
 } /* namespace */
 
-/* the same buffer cache for the library's other translation units (merge.cu) */
+/* the same buffer cache for the library's other translation units (scan.h) */
 cudaError_t dng_cached_alloc(int device, void **p, size_t n)
 {
 	return cached_alloc(device, p, n);
@@ -148,140 +141,6 @@ void dng_cached_free(void *p)
 {
 	cached_free(p);
 }
-
-
-struct dng_scan {
-	dng_plan plan;
-	int device = 0;
-	int sm_count = 0;
-	u32 plan_bytes = 0, sslots = 0, s1slots = 0;
-	cudaStream_t stream = nullptr, copy_stream = nullptr;
-	cudaStream_t own_stream = nullptr;
-	DevPlan *d_plan = nullptr;
-	GTable tab{};
-	unsigned long long *d_counters = nullptr;
-	unsigned long long *d_nl = nullptr;	/* find_nl scratch (2) */
-	size_t table_cap = 0;
-	/* H2D ring */
-	size_t ring_cap = 0;
-	u8 *d_ring[RING_SLOTS] = {};
-	u8 *h_stage[RING_SLOTS] = {};
-	cudaEvent_t ev_ready[RING_SLOTS] = {}, ev_free[RING_SLOTS] = {};
-	bool slot_used[RING_SLOTS] = {};
-	size_t next_slot = 0;
-	/* carry: the unterminated tail of everything fed so far */
-	u8 *d_carry = nullptr;
-	size_t carry_len = 0;
-	u8 *d_side = nullptr;		/* carry + head of a device chunk */
-	/* pinned block ring of dng_scan_feed_file's reader threads */
-	u8 *file_buf = nullptr;
-	cudaEvent_t file_done[32] = {};
-	/* dng_scan_read_stats */
-	uint64_t direct_bytes = 0, buffered_bytes = 0, direct_ranges = 0;
-	uint64_t read_fallbacks = 0;
-	/* dng_scan_feed_gzip and dng_scan_feed_bzip2: compressed files queued
-	 * for the next batch, all of one format (path, compressed size, output
-	 * room of a gzip file), and the batch's compressed bytes */
-	struct CzFile {
-		std::string path;
-		size_t size;
-		uint64_t hint;
-		uint32_t head;		/* a bzip2 file's first four bytes */
-	};
-	std::vector<CzFile> cz_queue;
-	bool cz_bzip2 = false;		/* the queue's format */
-	uint64_t cz_queued_in = 0, cz_queued_out = 0;
-	/* the gzip path's device buffers and stats */
-	u8 *d_cz_in = nullptr, *d_gz_out = nullptr, *d_gz_big = nullptr;
-	u8 *d_gz_join = nullptr;
-	size_t cz_in_cap = 0, gz_out_cap = 0, gz_big_cap = 0, gz_join_cap = 0;
-	u8 *d_gz_jobs = nullptr, *h_gz_jobs = nullptr;	/* jobs, results, next */
-	uint64_t gz_files = 0, gz_members = 0, gz_in_bytes = 0, gz_out_bytes = 0;
-	uint64_t gz_launches = 0;
-	double gz_ms = 0;
-	/* the split path (inflate_split.cuh): a batch's chunk state, symbols,
-	 * outputs that missed their regions and checks; its stats */
-	u8 *d_gz_split = nullptr, *d_gz_sym = nullptr, *d_gz_sout = nullptr;
-	u8 *d_gz_check = nullptr;
-	size_t gz_split_cap = 0, gz_sym_cap = 0, gz_sout_cap = 0;
-	size_t gz_check_cap = 0;
-	uint64_t gz_split_files = 0, gz_chunks = 0, gz_false_starts = 0;
-	uint64_t gz_fallbacks = 0, gz_split_launches = 0;
-	uint32_t gz_split_blocks = 0;	/* CTAs of split_decode_kernel per SM */
-	/* the bzip2 path (bunzip.cuh): candidates, BWT slots, transformation
-	 * vectors, per-block records and output of a wave; its stats */
-	u8 *d_bz_find = nullptr, *d_bz_slot = nullptr, *d_bz_tt = nullptr;
-	u8 *d_bz_rec = nullptr, *d_bz_out = nullptr;
-	size_t bz_find_cap = 0, bz_slot_cap = 0, bz_tt_cap = 0, bz_rec_cap = 0;
-	size_t bz_out_cap = 0;
-	uint64_t bz_files = 0, bz_streams = 0, bz_blocks = 0;
-	uint64_t bz_false_starts = 0, bz_in_bytes = 0, bz_out_bytes = 0;
-	uint64_t bz_launches = 0;
-	double bz_ms = 0;
-	double bz_stage_ms[4] = {};	/* find, decode, invert, emit */
-	/* stats */
-	std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev_pairs;
-	std::vector<cudaEvent_t> ev_pool;
-	double kernel_ms = 0;
-	uint64_t launches = 0, kernel_bytes = 0, bytes_fed = 0;
-	uint64_t aux_launches = 0;	/* resolve / find_nl / compact kernels */
-	cudaEvent_t ev_init = nullptr;	/* setup enqueued by dng_scan_open */
-	bool finished = false;
-	/* record templates (tmpl.h), learned from the head of the input */
-	bool tmpl_enabled = true, tmpl_tried = false;
-	KernelChoice kc;		/* which kernel, at what geometry */
-	u32 w_sslots = 0, w_s1slots = 0;
-	/* counters of finished launches, copied to pinned memory after every
-	 * launch: lets the host notice that the input changed character */
-	unsigned long long *h_live = nullptr;
-	u8 *d_tmpl = nullptr;
-	u32 tmpl_bytes = 0, ntemplates = 0;
-	/* what learns since d_tmpl was last built resolved, oldest first: the
-	 * first general launch builds d_tmpl from it (an F scan never does) */
-	std::vector<std::pair<std::vector<TCandidate>, std::vector<TResolved>>>
-	    tmpl_pending;
-	u8 *h_blobs = nullptr;		/* pinned staging of the blob uploads */
-	/* the F path (fast.h): its plan, its templates, its miss list */
-	FPlan fplan;
-	FPlan *d_fplan = nullptr;
-	u8 *d_ftmpl = nullptr;
-	u32 ftmpl_bytes = 0, nftemplates = 0, ftmpl_leaf_off = 0, ftmpl_pool_off = 0;
-	u32 f_smem_max = 0;		/* dynamic shared memory a CTA may ask for */
-	/* run-time compiled matcher (jit.h): 0 off, 1 in the background, 2 wait */
-	int jit_mode = 1;
-	std::shared_ptr<JitKernels> jit;
-	uint64_t jit_launches = 0;
-	MissEnt *d_miss = nullptr;
-	u32 *d_miss_n = nullptr;
-	u32 miss_cap = 0;
-	unsigned long long seen_tmpl = 0;
-	/* a scan over several devices (dng_scan_open_devices) holds no device
-	 * state of its own: it records the files fed, with their sizes, and
-	 * at finish cuts them into one byte range per shard */
-	bool multi = false;
-	std::vector<dng_scan *> shards;
-	std::vector<std::pair<std::string, size_t>> files;
-	std::string err;
-	int err_code = 0;
-
-	int fail(int code, const std::string &m) {
-		if (!err_code) {
-			err_code = code;
-			err = m;
-		}
-		return code;
-	}
-	int cuda(cudaError_t e, const char *what) {
-		if (e == cudaSuccess)
-			return 0;
-		return fail(DNG_ECUDA, std::string(what) + ": " +
-		    cudaGetErrorString(e));
-	}
-};
-
-#define CK(s, call) do { if ((s)->cuda((call), #call)) return (s)->err_code; } while (0)
-
-namespace {
 
 cudaEvent_t get_event(dng_scan *s)
 {
@@ -294,6 +153,8 @@ cudaEvent_t get_event(dng_scan *s)
 	cudaEventCreate(&e);
 	return e;
 }
+
+namespace {
 
 /* shared memory set aside for the template trie when sizing the tally cache */
 static constexpr size_t TMPL_RESERVE = 4096;
@@ -858,8 +719,6 @@ int feed_host(dng_scan *s, const void *vbuf, size_t len, bool pinned)
 
 } /* namespace */
 
-extern "C" {
-
 const char *dng_version(void)
 {
 	return "dragnet-b200 0.1 (sm_90a)";
@@ -1123,7 +982,7 @@ dng_scan *dng_scan_shard(const dng_scan *s, int i)
 }
 
 /* what a multi-device scan refuses: not sticky, the scan goes on */
-static int refuse_multi(dng_scan *s, const char *what)
+int refuse_multi(dng_scan *s, const char *what)
 {
 	if (!s->err_code)
 		s->err = std::string(what) + " on a scan over several devices "
@@ -1143,9 +1002,6 @@ int dng_scan_set_stream(dng_scan *s, void *cuda_stream)
 	CK(s, cudaStreamWaitEvent(s->stream, s->ev_init, 0));
 	return DNG_OK;
 }
-
-static int cz_flush(dng_scan *s);
-static int feed_device(dng_scan *s, const void *devbuf, size_t len);
 
 static int ensure_ring(dng_scan *s, bool need_stage)
 {
@@ -1357,7 +1213,7 @@ static int feed_file_parallel(dng_scan *s, int fd, size_t off, size_t size,
 		}
 		if (rc)
 			break;
-		if (bytes && to_dev) {	/* (a gzip file: to its batch buffer) */
+		if (bytes && to_dev) {	/* (a compressed file: to its batch) */
 			rc = s->cuda(cudaMemcpyAsync(to_dev, s->file_buf +
 			    (b % NSLOT) * BLK + r.plan.lo(b), bytes,
 			    cudaMemcpyHostToDevice, s->copy_stream),
@@ -1396,6 +1252,20 @@ static int feed_file_parallel(dng_scan *s, int fd, size_t off, size_t size,
 	s->read_fallbacks += r.fallbacks;
 	/* the pinned ring is reused by the next file: drain its copies */
 	cudaStreamSynchronize(s->copy_stream);
+	return rc;
+}
+
+/* bytes [0, size) of the file at `path` to device memory at `dst`, through
+ * the reader above (a compressed file, to its batch buffer); a file that is
+ * now shorter fails with DNG_EIO */
+int read_to_device(dng_scan *s, const char *path, size_t size, u8 *dst)
+{
+	int fd = open(path, O_RDONLY);
+	if (fd < 0)
+		return s->fail(DNG_EIO, std::string("open ") + path + ": " +
+		    strerror(errno));
+	const int rc = feed_file_parallel(s, fd, 0, size, path, true, dst);
+	close(fd);
 	return rc;
 }
 
@@ -1643,8 +1513,9 @@ int dng_scan_feed_device(dng_scan *s, const void *devbuf, size_t len)
 	return feed_device(s, devbuf, len);
 }
 
-/* dng_scan_feed_device of a single-device scan with no gzip files queued */
-static int feed_device(dng_scan *s, const void *devbuf, size_t len)
+/* dng_scan_feed_device of a single-device scan with no compressed files
+ * queued */
+int feed_device(dng_scan *s, const void *devbuf, size_t len)
 {
 	if (s->err_code)
 		return s->err_code;
@@ -1763,1202 +1634,6 @@ static int feed_device(dng_scan *s, const void *devbuf, size_t len)
 		s->carry_len = tail;
 	}
 	return 0;
-}
-
-/* ---- gzip files (dng_scan_feed_gzip) -------------------------------------
- *
- * Queued files are inflated in batches by inflate_kernel (inflate.cuh), one
- * warp per file, into output regions laid out back to back in one device
- * buffer, each as large as its file's ISIZE trailer says (exact for a single
- * member under 4 GiB).  When every file filled its region exactly, the batch
- * is fed as one device buffer (one newline search, one wait).  Otherwise
- * each run of files that filled their regions is fed as one buffer, each file
- * that did not on its own, and a file that ran out of room is decoded again,
- * alone, in twice the room until it fits (several members, trailing zeros, or
- * >= 4 GiB).
- *
- * A batch holds at most 2 GiB of output room, 512 MiB of compressed bytes
- * and 256 files; a larger file goes alone.  One warp decodes one file, except
- * the large files of a batch of few, which are split (below).  Its buffers
- * (2.5 GiB) live beside the scan's own (table, arena, H2D ring: about
- * 2.5 GiB at the defaults), far below an H100's 80 GB.  Every batch buffer is written on the
- * scan's stream, after the scan kernels that read it earlier: a region stays
- * valid until those kernels have finished, as dng_scan_feed_device needs.
- */
-static const size_t GZ_BATCH_OUT = (size_t)2 << 30;
-static const size_t GZ_BATCH_IN = (size_t)512 << 20;
-static const size_t GZ_BATCH_FILES = 256;
-
-static size_t round16(size_t n)
-{
-	return (n + 15) & ~(size_t)15;
-}
-
-/* make *p hold at least n bytes (powers of two from 1 MiB, so the buffer
- * cache takes them back); what the old buffer held is not kept */
-static int gz_room(dng_scan *s, u8 **p, size_t *cap, size_t n)
-{
-	if (*p && *cap >= n)
-		return 0;
-	size_t c = (size_t)1 << 20;
-	while (c < n)
-		c <<= 1;
-	if (*p) {
-		/* scan kernels enqueued earlier may still read it */
-		CK(s, cudaStreamSynchronize(s->stream));
-		cached_free(*p);
-		*p = nullptr;
-		*cap = 0;
-	}
-	CK(s, DEV_ALLOC(s, p, c));
-	*cap = c;
-	return 0;
-}
-
-/* one inflate launch over jobs[0, n) on the scan's stream, and its results:
- * the one wait of a batch */
-static int gz_launch(dng_scan *s, const InfJob *jobs, u32 n, InfResult *out)
-{
-	const size_t jb = GZ_BATCH_FILES * sizeof (InfJob);
-	const size_t rb = GZ_BATCH_FILES * sizeof (InfResult);
-	if (!s->d_gz_jobs) {
-		CK(s, DEV_ALLOC(s, &s->d_gz_jobs, jb + rb + 64));
-		CK(s, HOST_ALLOC(&s->h_gz_jobs, jb + rb));
-	}
-	memcpy(s->h_gz_jobs, jobs, n * sizeof (InfJob));
-	CK(s, cudaMemcpyAsync(s->d_gz_jobs, s->h_gz_jobs, n * sizeof (InfJob),
-	    cudaMemcpyHostToDevice, s->stream));
-	u32 *d_next = (u32 *)(s->d_gz_jobs + jb + rb);
-	CK(s, cudaMemsetAsync(d_next, 0, sizeof (u32), s->stream));
-	cudaEvent_t e0 = get_event(s), e1 = get_event(s);
-	cudaEventRecord(e0, s->stream);
-	const u32 grid = std::min<u32>((n + INF_WARPS - 1) / INF_WARPS,
-	    (u32)s->sm_count * 4);
-	inflate_kernel<<<grid, 32 * INF_WARPS, 0, s->stream>>>(
-	    (const InfJob *)s->d_gz_jobs, (InfResult *)(s->d_gz_jobs + jb), n,
-	    d_next);
-	cudaError_t e = cudaGetLastError();
-	cudaEventRecord(e1, s->stream);
-	s->aux_launches++;
-	s->gz_launches++;
-	if (e == cudaSuccess)
-		e = cudaMemcpyAsync(s->h_gz_jobs + jb, s->d_gz_jobs + jb,
-		    n * sizeof (InfResult), cudaMemcpyDeviceToHost, s->stream);
-	if (e == cudaSuccess)
-		e = cudaStreamSynchronize(s->stream);
-	float ms = 0;
-	if (e == cudaSuccess && cudaEventElapsedTime(&ms, e0, e1) == cudaSuccess)
-		s->gz_ms += ms;
-	/* (back to the pool on every path: the stream is synchronized or
-	 * failed, and dng_scan_destroy waits for it before freeing them) */
-	s->ev_pool.push_back(e0);
-	s->ev_pool.push_back(e1);
-	if (s->cuda(e, "inflate_kernel"))
-		return s->err_code;
-	memcpy(out, s->h_gz_jobs + jb, n * sizeof (InfResult));
-	return 0;
-}
-
-static int gz_damage(dng_scan *s, const std::string &path, const InfResult &r)
-{
-	return s->fail(DNG_EIO, path + ": corrupt gzip data: " +
-	    inflate_error_name(r.kind) + " (compressed byte " +
-	    std::to_string(r.bit / 8) + ")");
-}
-
-/* ---- gzip files split into chunks (inflate_split.cuh) ----------------------
- *
- * A batch with fewer files than the device holds decode warps cuts its large
- * files into chunks (gz_split_plan, inflate_policy.h).  Before the batch's
- * one wait: split_find_kernel finds each chunk's candidate block start and
- * split_decode_kernel decodes every chunk into 16-bit symbols.  After it the
- * host chains each file's chunks; a chain that ends in a chunk out of room
- * decodes that chunk, and each later one that ran out, again in four times
- * the room and member slots.  Then split_tail_kernel and split_body_kernel
- * write each file's bytes, into its region when its length is the hint and
- * into d_gz_sout otherwise, and split_crc_kernel and split_member_kernel
- * check every member.  A file the split path cannot vouch for is decoded
- * again by inflate_kernel, whose answer stands.
- *
- * Scratch, from the buffer cache: 16-bit symbols for 1.25 times each split
- * file's hint plus 32 Ki symbols per chunk (2.5 times the batch's output
- * room, plus 64 KiB per chunk), and four times that for each chunk decoded
- * again; per chunk its candidate, job, result and four member slots; the
- * pieces and members of the checks.
- */
-struct GzChunk {		/* host state of one chunk */
-	SplitJob job;
-	SplitRes res;
-	std::vector<InfMember> mem;
-};
-
-struct GzSplitFile {
-	size_t file;			/* in the batch */
-	uint32_t first, n;		/* its chunks in the batch's list */
-	int chain;
-	std::vector<uint32_t> proven;
-	SplitLayout lay;
-	u8 *dst;
-	bool ok;
-};
-
-static uint64_t gz_resident(dng_scan *s)
-{
-	if (!s->gz_split_blocks) {
-		int b = 0;
-		cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b,
-		    split_decode_kernel, 32 * SPLIT_WARPS, 0);
-		s->gz_split_blocks = b > 0 ? (uint32_t)b : 1;
-	}
-	return (uint64_t)s->gz_split_blocks * SPLIT_WARPS * s->sm_count;
-}
-
-/* time a stretch of split kernels into inflate_ms, once the stream is idle */
-struct GzTimer {
-	cudaEvent_t e0, e1;
-};
-
-static GzTimer gz_timer_start(dng_scan *s)
-{
-	GzTimer t = { get_event(s), get_event(s) };
-	cudaEventRecord(t.e0, s->stream);
-	return t;
-}
-
-static void gz_timer_stop(dng_scan *s, GzTimer &t)
-{
-	cudaEventRecord(t.e1, s->stream);
-}
-
-static void gz_timer_read(dng_scan *s, GzTimer &t)
-{
-	float ms = 0;
-	if (cudaEventElapsedTime(&ms, t.e0, t.e1) == cudaSuccess)
-		s->gz_ms += ms;
-	s->ev_pool.push_back(t.e0);
-	s->ev_pool.push_back(t.e1);
-}
-
-static void gz_split_count(dng_scan *s, uint32_t launches)
-{
-	s->gz_split_launches += launches;
-	s->aux_launches += launches;
-}
-
-/* split_decode_kernel over the chunks `which` (their jobs set), on the
- * stream; device records at d_jobs / d_res */
-static int gz_split_decode(dng_scan *s, std::vector<GzChunk> &ck,
-    const std::vector<uint32_t> &which, u8 *d_jobs, u8 *d_res, u32 *d_next)
-{
-	const size_t n = which.size();
-	std::vector<SplitJob> jobs(n);
-	for (size_t i = 0; i < n; i++)
-		jobs[i] = ck[which[i]].job;
-	CK(s, cudaMemcpyAsync(d_jobs, jobs.data(), n * sizeof (SplitJob),
-	    cudaMemcpyHostToDevice, s->stream));
-	CK(s, cudaMemsetAsync(d_next, 0, sizeof (u32), s->stream));
-	gz_resident(s);
-	const u32 grid = std::min<u32>((u32)((n + SPLIT_WARPS - 1) / SPLIT_WARPS),
-	    s->gz_split_blocks * (u32)s->sm_count);
-	split_decode_kernel<<<grid, 32 * SPLIT_WARPS, 0, s->stream>>>(
-	    (const SplitJob *)d_jobs, (SplitRes *)d_res, (u32)n, d_next);
-	gz_split_count(s, 1);
-	CK(s, cudaGetLastError());
-	return 0;
-}
-
-/* 1 and 2: enqueue the finder and the first decode of every chunk of the
- * split files (no wait) */
-static int gz_split_start(dng_scan *s, const std::vector<dng_scan::CzFile> &q,
-    const std::vector<size_t> &in_off, const std::vector<u32> &nch,
-    std::vector<GzSplitFile> &sf, std::vector<GzChunk> &ck, GzTimer &t)
-{
-	uint32_t total = 0;
-	uint64_t room = 0;
-	for (size_t i = 0; i < q.size(); i++) {
-		if (nch[i] < 2)
-			continue;
-		GzSplitFile f = {};
-		f.file = i;
-		f.first = total;
-		f.n = nch[i];
-		sf.push_back(f);
-		total += nch[i];
-	}
-	ck.resize(total);
-	for (const GzSplitFile &f : sf) {
-		const dng_scan::CzFile &g = q[f.file];
-		for (uint32_t k = 0; k < f.n; k++) {
-			const uint64_t cb = split_cut(g.size, f.n, k + 1) -
-			    split_cut(g.size, f.n, k);
-			SplitJob &j = ck[f.first + k].job;
-			j = {};
-			j.in = s->d_cz_in + in_off[f.file];
-			j.in_len = g.size;
-			j.cap = split_room(g.hint, g.size, cb);
-			j.k = k;
-			j.nchunks = f.n;
-			j.mcap = SPLIT_MSLOTS;
-			room += j.cap;
-		}
-	}
-	/* candidates | find jobs | decode jobs | results | member slots | next */
-	const size_t oc = 0, of = oc + total * sizeof (uint64_t),
-	    oj = of + total * sizeof (SplitFind),
-	    orr = oj + total * sizeof (SplitJob),
-	    om = orr + total * sizeof (SplitRes),
-	    on = om + (size_t)total * SPLIT_MSLOTS * sizeof (InfMember);
-	if (gz_room(s, &s->d_gz_split, &s->gz_split_cap, on + 16) ||
-	    gz_room(s, &s->d_gz_sym, &s->gz_sym_cap, room * 2))
-		return s->err_code;
-	uint64_t *d_cand = (uint64_t *)(s->d_gz_split + oc);
-	std::vector<SplitFind> finds;
-	uint64_t sym = 0;
-	for (const GzSplitFile &f : sf) {
-		const dng_scan::CzFile &g = q[f.file];
-		for (uint32_t k = 0; k < f.n; k++) {
-			SplitJob &j = ck[f.first + k].job;
-			j.cand = d_cand + f.first;
-			j.out = (uint16_t *)s->d_gz_sym + sym;
-			j.mem = (InfMember *)(s->d_gz_split + om) +
-			    (size_t)(f.first + k) * SPLIT_MSLOTS;
-			sym += j.cap;
-			if (k)
-				finds.push_back({ j.in, g.size,
-				    split_cut(g.size, f.n, k) * 8,
-				    split_cut(g.size, f.n, k + 1) * 8,
-				    d_cand + f.first + k });
-		}
-	}
-	CK(s, cudaMemcpyAsync(s->d_gz_split + of, finds.data(),
-	    finds.size() * sizeof (SplitFind), cudaMemcpyHostToDevice,
-	    s->stream));
-	t = gz_timer_start(s);
-	const u32 grid = std::min<u32>((u32)finds.size(), (u32)s->sm_count * 6);
-	split_find_kernel<<<grid, 32, 0, s->stream>>>(
-	    (const SplitFind *)(s->d_gz_split + of), (u32)finds.size());
-	gz_split_count(s, 1);
-	CK(s, cudaGetLastError());
-	std::vector<uint32_t> all(total);
-	for (uint32_t c = 0; c < total; c++)
-		all[c] = c;
-	if (gz_split_decode(s, ck, all, s->d_gz_split + oj,
-	    s->d_gz_split + orr, (u32 *)(s->d_gz_split + on)))
-		return s->err_code;
-	gz_timer_stop(s, t);
-	return 0;
-}
-
-/* results of chunks `which`, decoded into d_res, and their member records
- * from the slots [d_mem, + nslots) their jobs point into */
-static int gz_split_collect(dng_scan *s, std::vector<GzChunk> &ck,
-    const std::vector<uint32_t> &which, const u8 *d_res,
-    const InfMember *d_mem, size_t nslots)
-{
-	std::vector<SplitRes> r(which.size());
-	std::vector<InfMember> m(nslots);
-	CK(s, cudaMemcpyAsync(r.data(), d_res, r.size() * sizeof (SplitRes),
-	    cudaMemcpyDeviceToHost, s->stream));
-	CK(s, cudaMemcpyAsync(m.data(), d_mem, nslots * sizeof (InfMember),
-	    cudaMemcpyDeviceToHost, s->stream));
-	CK(s, cudaStreamSynchronize(s->stream));
-	for (size_t i = 0; i < which.size(); i++) {
-		GzChunk &c = ck[which[i]];
-		c.res = r[i];
-		const InfMember *h = m.data() + (c.job.mem - d_mem);
-		c.mem.assign(h, h + c.res.members);
-	}
-	return 0;
-}
-
-/*
- * 3 to 5, after the batch's wait: chain, decode again what ran out of room,
- * resolve and check.  by_file[i] of a split file: DONE with its length and
- * members (alt[i]: where its bytes are when not in its region), or ROOM,
- * to be decoded whole (a fallback).
- */
-static int gz_split_finish(dng_scan *s, const std::vector<dng_scan::CzFile> &q,
-    const std::vector<size_t> &out_off, std::vector<GzSplitFile> &sf,
-    std::vector<GzChunk> &ck, std::vector<InfResult> &by_file,
-    std::vector<const u8 *> &alt)
-{
-	std::vector<uint32_t> all(ck.size());
-	for (uint32_t c = 0; c < ck.size(); c++)
-		all[c] = c;
-	const size_t orr = ck.size() * (sizeof (uint64_t) + sizeof (SplitFind) +
-	    sizeof (SplitJob)), om = orr + ck.size() * sizeof (SplitRes);
-	if (gz_split_collect(s, ck, all, s->d_gz_split + orr,
-	    (const InfMember *)(s->d_gz_split + om), ck.size() * SPLIT_MSLOTS))
-		return s->err_code;
-	std::vector<u8 *> extra;	/* rooms of chunks decoded again */
-	struct Free {
-		std::vector<u8 *> &v;
-		~Free() { for (u8 *p : v) cached_free(p); }
-	} free_extra = { extra };
-	for (;;) {
-		std::vector<uint32_t> redo, r;
-		for (GzSplitFile &f : sf) {
-			std::vector<SplitRes> res(f.n);
-			for (uint32_t k = 0; k < f.n; k++)
-				res[k] = ck[f.first + k].res;
-			f.chain = split_chain(res.data(), f.proven);
-			if (f.chain != CHAIN_ROOM)
-				continue;
-			split_redo(res.data(), f.n, f.proven, r);
-			for (const uint32_t k : r)
-				redo.push_back(f.first + k);
-		}
-		if (redo.empty())
-			break;
-		uint64_t room = 0, slots = 0;
-		for (const uint32_t c : redo) {
-			room += ck[c].job.cap * 4;
-			slots += ck[c].job.mcap * 4;
-		}
-		const size_t bj = redo.size() * sizeof (SplitJob),
-		    br = redo.size() * sizeof (SplitRes),
-		    bm = slots * sizeof (InfMember);
-		u8 *d = nullptr;
-		CK(s, DEV_ALLOC(s, &d, room * 2 + bj + br + bm + 16));
-		extra.push_back(d);
-		uint64_t sym = 0, slot = 0;
-		for (const uint32_t c : redo) {
-			SplitJob &j = ck[c].job;
-			j.cap *= 4;
-			j.mcap *= 4;
-			j.out = (uint16_t *)d + sym;
-			j.mem = (InfMember *)(d + room * 2 + bj + br) + slot;
-			sym += j.cap;
-			slot += j.mcap;
-		}
-		GzTimer t = gz_timer_start(s);
-		if (gz_split_decode(s, ck, redo, d + room * 2, d + room * 2 + bj,
-		    (u32 *)(d + room * 2 + bj + br + bm)))
-			return s->err_code;
-		gz_timer_stop(s, t);
-		const int rc = gz_split_collect(s, ck, redo, d + room * 2 + bj,
-		    (const InfMember *)(d + room * 2 + bj + br), slots);
-		gz_timer_read(s, t);
-		if (rc)
-			return rc;
-	}
-	/* lay out every file whose chain reached the end */
-	size_t sout = 0;
-	for (GzSplitFile &f : sf) {
-		f.ok = f.chain == CHAIN_END;
-		s->gz_split_files++;
-		s->gz_chunks += f.n;
-		if (!f.ok)
-			continue;
-		std::vector<SplitRes> res(f.n);
-		std::vector<const InfMember *> mem(f.n);
-		for (uint32_t k = 0; k < f.n; k++) {
-			res[k] = ck[f.first + k].res;
-			mem[k] = ck[f.first + k].mem.data();
-		}
-		s->gz_false_starts += split_false_starts(res.data(), f.n,
-		    f.proven);
-		split_layout(res.data(), mem.data(), f.proven, f.lay);
-		if (f.lay.len != q[f.file].hint)
-			sout += round16(f.lay.len);
-	}
-	if (sout && gz_room(s, &s->d_gz_sout, &s->gz_sout_cap, sout))
-		return s->err_code;
-	/* resolve pieces | first | bad | CRC pieces | CRCs | members */
-	std::vector<SplitPiece> pieces;
-	std::vector<u32> first;
-	std::vector<CrcPiece> cp;
-	std::vector<CrcMember> cm;
-	std::vector<GzSplitFile *> okf;
-	sout = 0;
-	for (GzSplitFile &f : sf) {
-		if (!f.ok)
-			continue;
-		const u32 fi = (u32)okf.size();
-		okf.push_back(&f);
-		if (f.lay.len == q[f.file].hint) {
-			f.dst = s->d_gz_out + out_off[f.file];
-		} else {
-			f.dst = s->d_gz_sout + sout;
-			sout += round16(f.lay.len);
-		}
-		first.push_back((u32)pieces.size());
-		for (size_t i = 0; i < f.proven.size(); i++) {
-			const GzChunk &c = ck[f.first + f.proven[i]];
-			pieces.push_back({ c.job.out, f.dst, f.lay.off[i],
-			    c.res.out_len, f.lay.minidx[i], fi });
-		}
-		for (size_t m = 0; m < f.lay.mstart.size(); m++) {
-			CrcMember x = { (u32)cp.size(), 0, f.lay.crc[m],
-			    f.lay.isize[m], f.lay.mend[m] - f.lay.mstart[m], fi,
-			    0 };
-			for (uint64_t a = f.lay.mstart[m]; a < f.lay.mend[m];
-			    a += SPLIT_CRC_PIECE)
-				cp.push_back({ f.dst + a, std::min<uint64_t>(
-				    SPLIT_CRC_PIECE, f.lay.mend[m] - a) });
-			x.p1 = (u32)cp.size();
-			cm.push_back(x);
-		}
-	}
-	first.push_back((u32)pieces.size());
-	const size_t nok = okf.size();
-	std::vector<u32> bad(nok, 0);
-	if (nok) {
-		const size_t o1 = pieces.size() * sizeof (SplitPiece),
-		    o2 = o1 + first.size() * sizeof (u32),
-		    o3 = (o2 + nok * sizeof (u32) + 15) & ~(size_t)15,
-		    o4 = o3 + cp.size() * sizeof (CrcPiece),
-		    o5 = (o4 + cp.size() * sizeof (u32) + 15) & ~(size_t)15,
-		    o6 = o5 + cm.size() * sizeof (CrcMember);
-		if (gz_room(s, &s->d_gz_check, &s->gz_check_cap, o6))
-			return s->err_code;
-		u8 *d = s->d_gz_check;
-		CK(s, cudaMemcpyAsync(d, pieces.data(), o1,
-		    cudaMemcpyHostToDevice, s->stream));
-		CK(s, cudaMemcpyAsync(d + o1, first.data(), o2 - o1,
-		    cudaMemcpyHostToDevice, s->stream));
-		CK(s, cudaMemsetAsync(d + o2, 0, nok * sizeof (u32), s->stream));
-		if (!cp.empty())
-			CK(s, cudaMemcpyAsync(d + o3, cp.data(), o4 - o3,
-			    cudaMemcpyHostToDevice, s->stream));
-		if (!cm.empty())
-			CK(s, cudaMemcpyAsync(d + o5, cm.data(), o6 - o5,
-			    cudaMemcpyHostToDevice, s->stream));
-		u32 *d_bad = (u32 *)(d + o2);
-		GzTimer t = gz_timer_start(s);
-		split_tail_kernel<<<(u32)nok, 1024, 0, s->stream>>>(
-		    (const SplitPiece *)d, (const u32 *)(d + o1), d_bad);
-		split_body_kernel<<<(u32)pieces.size(), 256, 0, s->stream>>>(
-		    (const SplitPiece *)d, d_bad);
-		gz_split_count(s, 2);
-		if (!cp.empty()) {
-			split_crc_kernel<<<(u32)((cp.size() + 255) / 256), 256, 0,
-			    s->stream>>>((const CrcPiece *)(d + o3),
-			    (u32 *)(d + o4), (u32)cp.size());
-			split_member_kernel<<<(u32)((cm.size() + 3) / 4), 128, 0,
-			    s->stream>>>((const CrcMember *)(d + o5),
-			    (u32)cm.size(), (const CrcPiece *)(d + o3),
-			    (const u32 *)(d + o4), d_bad);
-			gz_split_count(s, 2);
-		}
-		gz_timer_stop(s, t);
-		CK(s, cudaGetLastError());
-		CK(s, cudaMemcpyAsync(bad.data(), d_bad, nok * sizeof (u32),
-		    cudaMemcpyDeviceToHost, s->stream));
-		CK(s, cudaStreamSynchronize(s->stream));
-		gz_timer_read(s, t);
-	}
-	for (size_t fi = 0; fi < nok; fi++)
-		okf[fi]->ok = !bad[fi];
-	for (const GzSplitFile &f : sf) {
-		InfResult &r = by_file[f.file];
-		r = {};
-		if (!f.ok) {
-			r.status = INF_ROOM;	/* decoded whole */
-			s->gz_fallbacks++;
-			continue;
-		}
-		r.status = INF_DONE;
-		r.out_len = f.lay.len;
-		r.members = (uint32_t)f.lay.mstart.size();
-		if (f.dst != s->d_gz_out + out_off[f.file])
-			alt[f.file] = f.dst;
-	}
-	return 0;
-}
-
-static int bz_batch(dng_scan *s, const std::vector<dng_scan::CzFile> &q,
-    const std::vector<size_t> &in_off);
-
-/* inflate and feed a batch of gzip files, whose compressed bytes are in
- * d_cz_in at in_off, in the order they were fed */
-static int gz_batch(dng_scan *s, const std::vector<dng_scan::CzFile> &q,
-    const std::vector<size_t> &in_off)
-{
-	const size_t n = q.size();
-	std::vector<size_t> out_off(n);
-	size_t tout = 0;
-	for (size_t i = 0; i < n; i++) {
-		out_off[i] = tout;
-		tout += q[i].hint;
-	}
-	if (gz_room(s, &s->d_gz_out, &s->gz_out_cap, tout))
-		return s->err_code;
-	/* large files of a batch of few: split (inflate_policy.h) */
-	std::vector<uint64_t> sizes(n);
-	for (size_t i = 0; i < n; i++)
-		sizes[i] = q[i].size;
-	std::vector<u32> nch(n);
-	gz_split_plan(sizes.data(), n, gz_resident(s), DNG_GZ_SPLIT_FLOOR,
-	    nch.data());
-	std::vector<GzSplitFile> sf;
-	std::vector<GzChunk> ck;
-	GzTimer st = {};
-	for (size_t i = 0; i < n; i++)
-		if (nch[i] > 1) {
-			if (gz_split_start(s, q, in_off, nch, sf, ck, st))
-				return s->err_code;
-			break;
-		}
-	/* the rest one warp each, largest first, so that no big file is left
-	 * running alone */
-	std::vector<u32> order;
-	for (size_t i = 0; i < n; i++)
-		if (nch[i] < 2)
-			order.push_back((u32)i);
-	std::stable_sort(order.begin(), order.end(), [&](u32 a, u32 b) {
-		return q[a].size > q[b].size;
-	});
-	auto whole = [&](const std::vector<u32> &files,
-	    std::vector<InfResult> &by) {
-		std::vector<InfJob> jobs(files.size());
-		std::vector<InfResult> res(files.size());
-		for (size_t k = 0; k < files.size(); k++) {
-			const u32 i = files[k];
-			jobs[k] = { s->d_cz_in + in_off[i], q[i].size,
-			    s->d_gz_out + out_off[i], q[i].hint };
-		}
-		if (gz_launch(s, jobs.data(), (u32)files.size(), res.data()))
-			return s->err_code;
-		for (size_t k = 0; k < files.size(); k++)
-			by[files[k]] = res[k];
-		return 0;
-	};
-	std::vector<InfResult> by_file(n);
-	std::vector<const u8 *> alt(n, nullptr);
-	if (!order.empty() && whole(order, by_file))
-		return s->err_code;
-	if (!sf.empty()) {
-		if (order.empty())
-			CK(s, cudaStreamSynchronize(s->stream));
-		gz_timer_read(s, st);
-		if (gz_split_finish(s, q, out_off, sf, ck, by_file, alt))
-			return s->err_code;
-		/* what the split path could not vouch for, decoded whole */
-		std::vector<u32> again;
-		for (const GzSplitFile &f : sf)
-			if (!f.ok)
-				again.push_back((u32)f.file);
-		if (!again.empty() && whole(again, by_file))
-			return s->err_code;
-	}
-	for (size_t i = 0; i < n; i++) {
-		if (by_file[i].status == INF_ERROR)
-			return gz_damage(s, q[i].path, by_file[i]);
-		s->gz_in_bytes += q[i].size;
-	}
-	s->gz_files += n;
-	/* in file order: each run of files that filled their regions exactly
-	 * is one feed (the whole batch when every hint held); a file that did
-	 * not is fed on its own, decoded again in more room if it ran out */
-	auto filled = [&](size_t i) {
-		return by_file[i].status == INF_DONE &&
-		    by_file[i].out_len == q[i].hint;
-	};
-	for (size_t i = 0, next; i < n; i = next) {
-		const u8 *src = s->d_gz_out + out_off[i];
-		uint64_t len = 0;
-		next = i + 1;
-		if (filled(i)) {
-			while (next < n && filled(next))
-				next++;
-			for (size_t k = i; k < next; k++) {
-				s->gz_members += by_file[k].members;
-				len += by_file[k].out_len;
-			}
-		} else {
-			InfResult r = by_file[i];
-			if (alt[i])	/* split, and not the hint's length */
-				src = alt[i];
-			uint64_t cap = q[i].hint;
-			while (r.status == INF_ROOM) {
-				cap = std::max<uint64_t>(cap * 2,
-				    (uint64_t)1 << 20);
-				if (gz_room(s, &s->d_gz_big, &s->gz_big_cap, cap))
-					return s->err_code;
-				const InfJob j = { s->d_cz_in + in_off[i],
-				    q[i].size, s->d_gz_big, cap };
-				if (gz_launch(s, &j, 1, &r))
-					return s->err_code;
-				src = s->d_gz_big;
-			}
-			if (r.status == INF_ERROR)
-				return gz_damage(s, q[i].path, r);
-			s->gz_members += r.members;
-			len = r.out_len;
-		}
-		s->gz_out_bytes += len;
-		if (!len)
-			continue;	/* (an empty file adds nothing) */
-		if ((uintptr_t)src & 15) {
-			/* regions start where the hints before them end: a run
-			 * after a file that missed its hint is realigned */
-			if (gz_room(s, &s->d_gz_join, &s->gz_join_cap, len))
-				return s->err_code;
-			CK(s, cudaMemcpyAsync(s->d_gz_join, src, len,
-			    cudaMemcpyDeviceToDevice, s->stream));
-			src = s->d_gz_join;
-		}
-		if (feed_device(s, src, len))
-			return s->err_code;
-	}
-	return 0;
-}
-
-/* read the queued compressed files to the device and decode and feed them,
- * in the order they were fed */
-static int cz_flush(dng_scan *s)
-{
-	if (s->cz_queue.empty())
-		return s->err_code;
-	std::vector<dng_scan::CzFile> q;
-	q.swap(s->cz_queue);
-	s->cz_queued_in = s->cz_queued_out = 0;
-	if (s->err_code)
-		return s->err_code;
-	const size_t n = q.size();
-	std::vector<size_t> in_off(n);
-	size_t tin = 0;
-	for (size_t i = 0; i < n; i++) {
-		in_off[i] = tin;
-		tin += round16(q[i].size);
-	}
-	if (gz_room(s, &s->d_cz_in, &s->cz_in_cap, tin))
-		return s->err_code;
-	/* compressed bytes through the file reader (direct_read.h's policy) */
-	for (size_t i = 0; i < n; i++) {
-		const char *path = q[i].path.c_str();
-		int fd = open(path, O_RDONLY);
-		if (fd < 0)
-			return s->fail(DNG_EIO, std::string("open ") + path +
-			    ": " + strerror(errno));
-		const int rc = feed_file_parallel(s, fd, 0, q[i].size, path, true,
-		    s->d_cz_in + in_off[i]);
-		close(fd);
-		if (rc)
-			return rc;
-	}
-	return s->cz_bzip2 ? bz_batch(s, q, in_off) : gz_batch(s, q, in_off);
-}
-
-/* ---- bzip2 files (dng_scan_feed_bzip2) -------------------------------------
- *
- * A batch (the queue's limits: 256 files, 512 MiB compressed) is decoded by
- * the stages of bunzip.cuh.  bz_find_kernel finds every candidate magic of
- * every file; after that wait the host sorts them per file and cuts the block
- * candidates into waves (bunzip_policy.h).  Per wave: bz_decode_kernel
- * decodes every candidate (one wait), the host advances each file's chain
- * through them, bz_ibwt_kernel inverts the chained blocks and sizes their
- * output (one wait), and bz_emit_kernel writes each group of blocks back to
- * back, files in feed order, with their CRCs (one wait per group).  A group
- * is fed as one device buffer once its CRCs hold.  Every buffer is written on
- * the scan's stream, after the scan kernels that read it earlier.
- */
-struct BzStage {
-	cudaEvent_t e0, e1;
-};
-
-static BzStage bz_stage_start(dng_scan *s)
-{
-	BzStage t = { get_event(s), get_event(s) };
-	cudaEventRecord(t.e0, s->stream);
-	return t;
-}
-
-/* the stage's kernels are launched: count them, close the timer */
-static void bz_stage_stop(dng_scan *s, BzStage &t, uint32_t launches)
-{
-	cudaEventRecord(t.e1, s->stream);
-	s->bz_launches += launches;
-	s->aux_launches += launches;
-}
-
-/* once the stream is idle (or failed): its time into bunzip_ms */
-static void bz_stage_read(dng_scan *s, BzStage &t, int stage)
-{
-	float ms = 0;
-	if (cudaEventElapsedTime(&ms, t.e0, t.e1) == cudaSuccess) {
-		s->bz_ms += ms;
-		s->bz_stage_ms[stage] += ms;
-	}
-	s->ev_pool.push_back(t.e0);
-	s->ev_pool.push_back(t.e1);
-}
-
-static int bz_damage(dng_scan *s, const std::string &path, uint32_t kind,
-    uint64_t bit)
-{
-	const std::string what = kind == BE_TRAILING ?
-	    std::string(bunzip_error_name(kind)) :
-	    std::string("corrupt bzip2 data: ") + bunzip_error_name(kind);
-	return s->fail(DNG_EIO, path + ": " + what + " (compressed byte " +
-	    std::to_string(bit / 8) + ")");
-}
-
-static size_t bz_align(size_t n)
-{
-	return (n + 255) & ~(size_t)255;
-}
-
-/* every candidate magic of the batch, sorted by file and bit, and each
- * file's one past its last nonzero byte */
-static int bz_find(dng_scan *s, const std::vector<dng_scan::CzFile> &q,
-    const std::vector<size_t> &in_off, std::vector<BzCand> &cand,
-    std::vector<unsigned long long> &nz)
-{
-	const size_t n = q.size();
-	uint64_t tin = 0, maxlen = 0;
-	std::vector<BzFile> files(n);
-	for (size_t i = 0; i < n; i++) {
-		files[i] = { s->d_cz_in + in_off[i], q[i].size };
-		tin += q[i].size;
-		maxlen = std::max<uint64_t>(maxlen, q[i].size);
-	}
-	const size_t o_nz = bz_align(n * sizeof (BzFile));
-	const size_t o_cnt = o_nz + bz_align(n * 8);
-	const size_t o_cand = o_cnt + 256;
-	size_t cap = tin / 512 + 4096;
-	uint32_t count = 0;
-	nz.assign(n, 0);
-	for (;;) {
-		if (gz_room(s, &s->d_bz_find, &s->bz_find_cap, o_cand +
-		    cap * sizeof (BzCand)))
-			return s->err_code;
-		CK(s, cudaMemcpyAsync(s->d_bz_find, files.data(),
-		    n * sizeof (BzFile), cudaMemcpyHostToDevice, s->stream));
-		CK(s, cudaMemsetAsync(s->d_bz_find + o_nz, 0, o_cand - o_nz,
-		    s->stream));
-		const uint64_t per = 256 * 16;	/* bytes per CTA and sweep */
-		const dim3 grid((u32)std::min<uint64_t>(std::max<uint64_t>(
-		    (maxlen + per - 1) / per, 1), 65535), (u32)n);
-		BzStage t = bz_stage_start(s);
-		bz_find_kernel<<<grid, 256, 0, s->stream>>>(
-		    (const BzFile *)s->d_bz_find,
-		    (BzCand *)(s->d_bz_find + o_cand), (u32)cap,
-		    (u32 *)(s->d_bz_find + o_cnt),
-		    (unsigned long long *)(s->d_bz_find + o_nz));
-		cudaError_t e = cudaGetLastError();
-		bz_stage_stop(s, t, 1);
-		if (e == cudaSuccess)
-			e = cudaMemcpyAsync(nz.data(), s->d_bz_find + o_nz, n * 8,
-			    cudaMemcpyDeviceToHost, s->stream);
-		if (e == cudaSuccess)
-			e = cudaMemcpyAsync(&count, s->d_bz_find + o_cnt, 4,
-			    cudaMemcpyDeviceToHost, s->stream);
-		if (e == cudaSuccess)
-			e = cudaStreamSynchronize(s->stream);
-		bz_stage_read(s, t, 0);
-		if (s->cuda(e, "bz_find_kernel"))
-			return s->err_code;
-		if (count <= cap)
-			break;
-		cap = count;	/* more candidates than room: find again */
-	}
-	cand.resize(count);
-	if (count) {
-		CK(s, cudaMemcpyAsync(cand.data(), s->d_bz_find + o_cand,
-		    count * sizeof (BzCand), cudaMemcpyDeviceToHost, s->stream));
-		CK(s, cudaStreamSynchronize(s->stream));
-	}
-	std::sort(cand.begin(), cand.end(), [](const BzCand &a,
-	    const BzCand &b) {
-		return a.file != b.file ? a.file < b.file : a.bit < b.bit;
-	});
-	return 0;
-}
-
-/* decode, chain, invert and emit a batch of bzip2 files (above) */
-static int bz_batch(dng_scan *s, const std::vector<dng_scan::CzFile> &q,
-    const std::vector<size_t> &in_off)
-{
-	const size_t n = q.size();
-	std::vector<BzCand> cand;
-	std::vector<unsigned long long> nz;
-	if (bz_find(s, q, in_off, cand, nz))
-		return s->err_code;
-	/* each file's candidates, and the block candidates in order */
-	std::vector<u32> fbeg(n + 1, 0), bidx, which(cand.size(), ~0u);
-	for (const BzCand &c : cand)
-		fbeg[c.file + 1]++;
-	for (size_t i = 0; i < n; i++)
-		fbeg[i + 1] += fbeg[i];
-	for (u32 i = 0; i < cand.size(); i++)
-		if (cand[i].kind == BZ_CAND_BLOCK) {
-			which[i] = (u32)bidx.size();
-			bidx.push_back(i);
-		}
-	std::vector<size_t> ends(bidx.size() + 1);
-	const size_t nw = bz_waves(bidx.size(), DNG_BZ_WAVE_BLOCKS,
-	    ends.data());
-	std::vector<BzChain> ch(n);
-	for (size_t i = 0; i < n; i++)
-		bz_chain_init(ch[i], q[i].size, nz[i], q[i].head);
-	std::vector<BzDecResult> res(bidx.size());
-	size_t f = 0;	/* the first file whose chain is not done */
-	for (size_t w = 0, lo = 0;; w++) {
-		const size_t hi = w < nw ? ends[w] : lo, wn = hi - lo;
-		size_t o = 0;
-		auto at = [&](size_t bytes) {
-			const size_t r = o;
-			o += bz_align(bytes);
-			return r;
-		};
-		const size_t o_dj = at(wn * sizeof (BzDecJob));
-		const size_t o_dr = at(wn * sizeof (BzDecResult));
-		const size_t o_hist = at(wn * 256 * 4), o_next = at(16);
-		const size_t o_bj = at(wn * sizeof (BzBwtJob));
-		const size_t o_br = at(wn * sizeof (BzBwtResult));
-		const size_t o_ck = at(wn * BZ_CHUNKS * 8);
-		const size_t o_ej = at(wn * sizeof (BzEmitJob));
-		const size_t o_crc = at(wn * 4);
-		u8 *rec = nullptr;
-		if (wn) {
-			/* decode the wave's candidates, one warp each */
-			if (gz_room(s, &s->d_bz_rec, &s->bz_rec_cap, o) ||
-			    gz_room(s, &s->d_bz_slot, &s->bz_slot_cap,
-			    wn * (size_t)BZ_SLOT))
-				return s->err_code;
-			rec = s->d_bz_rec;
-			std::vector<BzDecJob> dj(wn);
-			for (size_t k = 0; k < wn; k++) {
-				const BzCand &c = cand[bidx[lo + k]];
-				dj[k] = { s->d_cz_in + in_off[c.file],
-				    q[c.file].size, c.bit,
-				    s->d_bz_slot + k * (size_t)BZ_SLOT,
-				    (uint32_t *)(rec + o_hist) + k * 256 };
-			}
-			CK(s, cudaMemcpyAsync(rec + o_dj, dj.data(),
-			    wn * sizeof (BzDecJob), cudaMemcpyHostToDevice,
-			    s->stream));
-			CK(s, cudaMemsetAsync(rec + o_next, 0, 16, s->stream));
-			const u32 grid = (u32)std::min<size_t>((wn + BZ_DEC_WARPS -
-			    1) / BZ_DEC_WARPS, (size_t)s->sm_count * 8);
-			BzStage t = bz_stage_start(s);
-			bz_decode_kernel<<<grid, 32 * BZ_DEC_WARPS, 0,
-			    s->stream>>>((const BzDecJob *)(rec + o_dj),
-			    (BzDecResult *)(rec + o_dr), (u32)wn,
-			    (u32 *)(rec + o_next));
-			cudaError_t e = cudaGetLastError();
-			bz_stage_stop(s, t, 1);
-			if (e == cudaSuccess)
-				e = cudaMemcpyAsync(res.data() + lo, rec + o_dr,
-				    wn * sizeof (BzDecResult),
-				    cudaMemcpyDeviceToHost, s->stream);
-			if (e == cudaSuccess)
-				e = cudaStreamSynchronize(s->stream);
-			bz_stage_read(s, t, 1);
-			if (s->cuda(e, "bz_decode_kernel"))
-				return s->err_code;
-		}
-		/* chain every file the decodes so far reach, in feed order; a
-		 * damaged file stops it, and fails the scan once the blocks
-		 * before the damage have passed their CRCs */
-		std::vector<u32> took;
-		bool early = false;
-		size_t damaged = n;
-		for (; f < n; f++) {
-			BzChain &c = ch[f];
-			const u32 b0 = fbeg[f];
-			bz_chain_run(c, cand.data() + b0, fbeg[f + 1] - b0,
-			    [&](u32 i) -> const BzDecResult * {
-				const size_t k = which[b0 + i];
-				return k < hi ? &res[k] : nullptr;
-			    }, [&](u32 i) {
-				early |= which[b0 + i] < lo;
-				took.push_back(which[b0 + i]);
-			    });
-			if (c.kind) {
-				damaged = f;
-				break;
-			}
-			if (early)
-				return s->fail(DNG_EIO, q[f].path + ": bzip2 "
-				    "chain went back to an earlier wave");
-			if (!c.done)
-				break;
-		}
-		s->bz_false_starts += wn - took.size();
-		const size_t m = took.size();
-		if (m) {
-			/* invert the chained blocks, one CTA each */
-			std::vector<size_t> tt_off(m);
-			size_t tsum = 0;
-			for (size_t k = 0; k < m; k++) {
-				tt_off[k] = tsum;
-				tsum += round16((size_t)res[took[k]].nblock * 4);
-			}
-			if (gz_room(s, &s->d_bz_tt, &s->bz_tt_cap, tsum))
-				return s->err_code;
-			std::vector<BzBwtJob> bj(m);
-			for (size_t k = 0; k < m; k++) {
-				const size_t c = took[k] - lo;
-				const BzDecResult &r = res[took[k]];
-				bj[k] = { s->d_bz_slot + c * (size_t)BZ_SLOT,
-				    (uint32_t *)(s->d_bz_tt + tt_off[k]),
-				    (const uint32_t *)(rec + o_hist) + c * 256,
-				    (uint32_t *)(rec + o_ck) + k * BZ_CHUNKS * 2,
-				    r.nblock, r.orig, r.rand, 0 };
-			}
-			CK(s, cudaMemcpyAsync(rec + o_bj, bj.data(),
-			    m * sizeof (BzBwtJob), cudaMemcpyHostToDevice,
-			    s->stream));
-			std::vector<BzBwtResult> br(m);
-			BzStage t = bz_stage_start(s);
-			bz_ibwt_kernel<<<(u32)m, BZ_THREADS, 0, s->stream>>>(
-			    (const BzBwtJob *)(rec + o_bj),
-			    (BzBwtResult *)(rec + o_br));
-			cudaError_t e = cudaGetLastError();
-			bz_stage_stop(s, t, 1);
-			if (e == cudaSuccess)
-				e = cudaMemcpyAsync(br.data(), rec + o_br,
-				    m * sizeof (BzBwtResult),
-				    cudaMemcpyDeviceToHost, s->stream);
-			if (e == cudaSuccess)
-				e = cudaStreamSynchronize(s->stream);
-			bz_stage_read(s, t, 2);
-			if (s->cuda(e, "bz_ibwt_kernel"))
-				return s->err_code;
-			std::vector<uint64_t> lens(m);
-			for (size_t k = 0; k < m; k++) {
-				const BzCand &c = cand[bidx[took[k]]];
-				if (!br[k].ok)	/* a run without its count */
-					return bz_damage(s, q[c.file].path,
-					    BE_OVERFLOW, c.bit);
-				lens[k] = br[k].out_len;
-			}
-			/* emit in groups, each fed once its CRCs hold */
-			std::vector<size_t> gend(m);
-			const size_t ng = bz_emit_groups(lens.data(), m,
-			    DNG_BZ_EMIT_OUT, gend.data());
-			for (size_t g = 0, g0 = 0; g < ng; g0 = gend[g++]) {
-				const size_t g1 = gend[g];
-				uint64_t sum = 0;
-				std::vector<BzEmitJob> ej(g1 - g0);
-				for (size_t k = g0; k < g1; k++)
-					sum += lens[k];
-				if (gz_room(s, &s->d_bz_out, &s->bz_out_cap, sum))
-					return s->err_code;
-				uint64_t off = 0;
-				for (size_t k = g0; k < g1; k++) {
-					ej[k - g0] = { bj[k].slot, bj[k].chunks,
-					    s->d_bz_out + off, bj[k].n, 0 };
-					off += lens[k];
-				}
-				CK(s, cudaMemcpyAsync(rec + o_ej, ej.data(),
-				    ej.size() * sizeof (BzEmitJob),
-				    cudaMemcpyHostToDevice, s->stream));
-				std::vector<uint32_t> crc(g1 - g0);
-				BzStage te = bz_stage_start(s);
-				bz_emit_kernel<<<(u32)(g1 - g0), BZ_THREADS, 0,
-				    s->stream>>>((const BzEmitJob *)(rec + o_ej),
-				    (uint32_t *)(rec + o_crc));
-				e = cudaGetLastError();
-				bz_stage_stop(s, te, 1);
-				if (e == cudaSuccess)
-					e = cudaMemcpyAsync(crc.data(), rec + o_crc,
-					    crc.size() * 4,
-					    cudaMemcpyDeviceToHost, s->stream);
-				if (e == cudaSuccess)
-					e = cudaStreamSynchronize(s->stream);
-				bz_stage_read(s, te, 3);
-				if (s->cuda(e, "bz_emit_kernel"))
-					return s->err_code;
-				for (size_t k = g0; k < g1; k++)
-					if (crc[k - g0] != res[took[k]].crc) {
-						const BzCand &c =
-						    cand[bidx[took[k]]];
-						return bz_damage(s,
-						    q[c.file].path,
-						    BE_BLOCK_CRC, c.bit);
-					}
-				s->bz_out_bytes += sum;
-				if (feed_device(s, s->d_bz_out, sum))
-					return s->err_code;
-			}
-		}
-		if (damaged < n)
-			return bz_damage(s, q[damaged].path, ch[damaged].kind,
-			    ch[damaged].err_bit);
-		lo = hi;
-		if (f == n) {
-			/* candidates past every chain's end: never decoded */
-			s->bz_false_starts += bidx.size() - hi;
-			break;
-		}
-		if (w >= nw)
-			return s->fail(DNG_EIO, q[f].path + ": bzip2 chain "
-			    "stopped before its end");
-	}
-	for (size_t i = 0; i < n; i++) {
-		s->bz_in_bytes += q[i].size;
-		s->bz_streams += ch[i].streams;
-		s->bz_blocks += ch[i].blocks;
-	}
-	s->bz_files += n;
-	return 0;
-}
-
-int dng_scan_feed_gzip(dng_scan *s, const char *path)
-{
-	if (!s || !path)
-		return DNG_EINVAL;
-	if (s->multi)
-		return refuse_multi(s, "dng_scan_feed_gzip");
-	if (s->err_code)
-		return s->err_code;
-	if (s->finished)
-		return s->fail(DNG_EINVAL, "scan already finished");
-	cudaSetDevice(s->device);
-	int fd = open(path, O_RDONLY);
-	if (fd < 0)
-		return s->fail(DNG_EIO, std::string("open ") + path + ": " +
-		    strerror(errno));
-	struct stat st;
-	u8 head[3] = {}, tail[4] = {};
-	const bool reg = fstat(fd, &st) == 0 && S_ISREG(st.st_mode);
-	const bool gz = reg && st.st_size >= 3 && pread(fd, head, 3, 0) == 3 &&
-	    head[0] == 0x1f && head[1] == 0x8b && head[2] == 8;
-	const bool trailer = gz && st.st_size >= 4 &&
-	    pread(fd, tail, 4, st.st_size - 4) == 4;
-	close(fd);
-	if (!gz) {
-		/* refused, not failed: the scan goes on */
-		if (!s->err_code)
-			s->err = std::string(path) + (reg ? ": not a gzip file "
-			    "(it does not start with 1f 8b 08)" :
-			    ": not a regular file");
-		return DNG_EINVAL;
-	}
-	const size_t size = (size_t)st.st_size;
-	const uint64_t hint = trailer ? inflate_hint(tail, size) : 0;
-	if (!s->cz_queue.empty() && (s->cz_bzip2 ||
-	    s->cz_queue.size() >= GZ_BATCH_FILES ||
-	    s->cz_queued_in + round16(size) > GZ_BATCH_IN ||
-	    s->cz_queued_out + hint > GZ_BATCH_OUT) && cz_flush(s))
-		return s->err_code;
-	s->cz_bzip2 = false;
-	s->cz_queue.push_back({ path, size, hint, 0 });
-	s->cz_queued_in += round16(size);
-	s->cz_queued_out += hint;
-	return DNG_OK;
-}
-
-int dng_scan_gzip_stats(dng_scan *s, uint64_t *files, uint64_t *members,
-    uint64_t *compressed_bytes, uint64_t *inflated_bytes, uint64_t *launches,
-    double *inflate_ms)
-{
-	if (!s)
-		return DNG_EINVAL;
-	if (files)
-		*files = s->gz_files;
-	if (members)
-		*members = s->gz_members;
-	if (compressed_bytes)
-		*compressed_bytes = s->gz_in_bytes;
-	if (inflated_bytes)
-		*inflated_bytes = s->gz_out_bytes;
-	if (launches)
-		*launches = s->gz_launches;
-	if (inflate_ms)
-		*inflate_ms = s->gz_ms;
-	return DNG_OK;
-}
-
-int dng_scan_gzip_split_stats(dng_scan *s, uint64_t *split_files,
-    uint64_t *chunks, uint64_t *false_starts, uint64_t *fallbacks,
-    uint64_t *launches)
-{
-	if (!s)
-		return DNG_EINVAL;
-	if (split_files)
-		*split_files = s->gz_split_files;
-	if (chunks)
-		*chunks = s->gz_chunks;
-	if (false_starts)
-		*false_starts = s->gz_false_starts;
-	if (fallbacks)
-		*fallbacks = s->gz_fallbacks;
-	if (launches)
-		*launches = s->gz_split_launches;
-	return DNG_OK;
-}
-
-int dng_scan_feed_bzip2(dng_scan *s, const char *path)
-{
-	if (!s || !path)
-		return DNG_EINVAL;
-	if (s->multi)
-		return refuse_multi(s, "dng_scan_feed_bzip2");
-	if (s->err_code)
-		return s->err_code;
-	if (s->finished)
-		return s->fail(DNG_EINVAL, "scan already finished");
-	cudaSetDevice(s->device);
-	int fd = open(path, O_RDONLY);
-	if (fd < 0)
-		return s->fail(DNG_EIO, std::string("open ") + path + ": " +
-		    strerror(errno));
-	struct stat st;
-	u8 h[4] = {};
-	const bool reg = fstat(fd, &st) == 0 && S_ISREG(st.st_mode);
-	const bool got = reg && st.st_size >= 4 && pread(fd, h, 4, 0) == 4;
-	close(fd);
-	const uint32_t head = (uint32_t)h[0] << 24 | (uint32_t)h[1] << 16 |
-	    (uint32_t)h[2] << 8 | h[3];
-	if (!got || !bz_level_ok(head)) {
-		/* refused, not failed: the scan goes on */
-		if (!s->err_code)
-			s->err = std::string(path) + (reg ? ": not a bzip2 file "
-			    "(it does not start with BZh and a level 1-9)" :
-			    ": not a regular file");
-		return DNG_EINVAL;
-	}
-	const size_t size = (size_t)st.st_size;
-	if (!s->cz_queue.empty() && (!s->cz_bzip2 ||
-	    s->cz_queue.size() >= GZ_BATCH_FILES ||
-	    s->cz_queued_in + round16(size) > GZ_BATCH_IN) && cz_flush(s))
-		return s->err_code;
-	s->cz_bzip2 = true;
-	s->cz_queue.push_back({ path, size, 0, head });
-	s->cz_queued_in += round16(size);
-	return DNG_OK;
-}
-
-int dng_scan_bzip2_stats(dng_scan *s, uint64_t *files, uint64_t *streams,
-    uint64_t *blocks, uint64_t *false_starts, uint64_t *compressed_bytes,
-    uint64_t *decompressed_bytes, uint64_t *launches, double *bunzip_ms)
-{
-	if (!s)
-		return DNG_EINVAL;
-	if (files)
-		*files = s->bz_files;
-	if (streams)
-		*streams = s->bz_streams;
-	if (blocks)
-		*blocks = s->bz_blocks;
-	if (false_starts)
-		*false_starts = s->bz_false_starts;
-	if (compressed_bytes)
-		*compressed_bytes = s->bz_in_bytes;
-	if (decompressed_bytes)
-		*decompressed_bytes = s->bz_out_bytes;
-	if (launches)
-		*launches = s->bz_launches;
-	if (bunzip_ms)
-		*bunzip_ms = s->bz_ms;
-	return DNG_OK;
-}
-
-int dng_scan_bzip2_stage_ms(dng_scan *s, double *find_ms, double *decode_ms,
-    double *invert_ms, double *emit_ms)
-{
-	if (!s)
-		return DNG_EINVAL;
-	double *const out[4] = { find_ms, decode_ms, invert_ms, emit_ms };
-	for (int i = 0; i < 4; i++)
-		if (out[i])
-			*out[i] = s->bz_stage_ms[i];
-	return DNG_OK;
 }
 
 int dng_scan_sync(dng_scan *s)
@@ -3200,8 +1875,7 @@ int dng_scan_template_stats(dng_scan *s, uint64_t *templates,
 		general_blob(s, blob, &nt);
 		*templates = blob.empty() ? s->ntemplates : nt;
 	}
-	if (templated_records)
-		*templated_records = c;
+	put(templated_records, c);
 	return DNG_OK;
 }
 
@@ -3229,14 +1903,10 @@ int dng_scan_read_stats(dng_scan *s, uint64_t *direct_bytes,
 		for (int i = 0; i < 4; i++)
 			v[i] += one[i];
 	}
-	if (direct_bytes)
-		*direct_bytes = v[0];
-	if (buffered_bytes)
-		*buffered_bytes = v[1];
-	if (direct_ranges)
-		*direct_ranges = v[2];
-	if (fallbacks)
-		*fallbacks = v[3];
+	put(direct_bytes, v[0]);
+	put(buffered_bytes, v[1]);
+	put(direct_ranges, v[2]);
+	put(fallbacks, v[3]);
 	return DNG_OK;
 }
 
@@ -3255,14 +1925,10 @@ int dng_scan_jit_stats(dng_scan *s, int *state, uint64_t *launches,
 	if (s->multi)
 		return refuse_multi(s, "dng_scan_jit_stats");
 	const int st = s->jit ? s->jit->state.load() : 0;
-	if (state)
-		*state = st;
-	if (launches)
-		*launches = s->jit_launches;
-	if (compile_ms)
-		*compile_ms = st ? s->jit->compile_ms : 0;
-	if (link_ms)
-		*link_ms = st ? s->jit->link_ms : 0;
+	put(state, st);
+	put(launches, s->jit_launches);
+	put(compile_ms, st ? s->jit->compile_ms : 0);
+	put(link_ms, st ? s->jit->link_ms : 0);
 	set_err(err, errlen, "%s", st == 2 ? s->jit->err.c_str() : "");
 	return DNG_OK;
 }
@@ -3277,12 +1943,9 @@ int dng_scan_kernel_stats(dng_scan *s, double *kernel_ms, uint64_t *launches,
 	cudaSetDevice(s->device);
 	if (dng_scan_sync(s))
 		return s->err_code;
-	if (kernel_ms)
-		*kernel_ms = s->kernel_ms;
-	if (launches)
-		*launches = s->launches;
-	if (kernel_bytes)
-		*kernel_bytes = s->kernel_bytes;
+	put(kernel_ms, s->kernel_ms);
+	put(launches, s->launches);
+	put(kernel_bytes, s->kernel_bytes);
 	return DNG_OK;
 }
 
@@ -3298,10 +1961,8 @@ int dng_scan_tally_stats(dng_scan *s, uint64_t *inline_overflow, int *f_warps)
 	unsigned long long c = 0;
 	CK(s, cudaMemcpy(&c, s->d_counters + CTR_OVER, sizeof (c),
 	    cudaMemcpyDeviceToHost));
-	if (inline_overflow)
-		*inline_overflow = c;
-	if (f_warps)
-		*f_warps = (int)s->kc.f_nw;
+	put(inline_overflow, c);
+	put(f_warps, (int)s->kc.f_nw);
 	return DNG_OK;
 }
 
@@ -3320,16 +1981,11 @@ int dng_jit_cache_stats(uint64_t *hits, uint64_t *misses, uint64_t *writes,
     uint64_t *evictions, uint64_t *errors)
 {
 	const dng::JitCacheStats st = dng::jit_cache_stats();
-	if (hits)
-		*hits = st.hits;
-	if (misses)
-		*misses = st.misses;
-	if (writes)
-		*writes = st.writes;
-	if (evictions)
-		*evictions = st.evictions;
-	if (errors)
-		*errors = st.errors;
+	put(hits, st.hits);
+	put(misses, st.misses);
+	put(writes, st.writes);
+	put(evictions, st.evictions);
+	put(errors, st.errors);
 	return DNG_OK;
 }
 
@@ -3403,21 +2059,7 @@ void dng_scan_destroy(dng_scan *s)
 	cached_free(s->d_nl);
 	cached_free(s->d_carry);
 	cached_free(s->d_side);
-	cached_free(s->d_cz_in);
-	cached_free(s->d_gz_out);
-	cached_free(s->d_gz_big);
-	cached_free(s->d_gz_join);
-	cached_free(s->d_gz_jobs);
-	cached_free(s->h_gz_jobs);
-	cached_free(s->d_gz_split);
-	cached_free(s->d_gz_sym);
-	cached_free(s->d_gz_sout);
-	cached_free(s->d_gz_check);
-	cached_free(s->d_bz_find);
-	cached_free(s->d_bz_slot);
-	cached_free(s->d_bz_tt);
-	cached_free(s->d_bz_rec);
-	cached_free(s->d_bz_out);
+	cz_free(s->cz);
 	if (s->own_stream)
 		cudaStreamDestroy(s->own_stream);
 	if (s->copy_stream)
@@ -3526,7 +2168,6 @@ int dng_gen_host(const dng_gen_params *p, uint64_t first, uint64_t count,
 	return DNG_OK;
 }
 
-} /* extern "C" */
 
 namespace {
 

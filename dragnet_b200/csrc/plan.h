@@ -188,6 +188,23 @@ static inline u32 devplan_smem_bytes(const DevPlan &p)
 	return (n + 127u) & ~127u;
 }
 
+/* the global tally table of a scan: the host allocates it, the scan kernels
+ * (scan_kernel.cuh) count into it */
+struct GEntry {
+	unsigned long long tag;		/* 0 empty, else hash | 1 */
+	unsigned long long count;
+	u32 koff;			/* key offset in arena + 1; 0 = unpublished */
+	u32 klen;
+};
+
+struct GTable {
+	GEntry *entries;
+	u8 *arena;
+	u32 *misc;			/* [0] arena cursor [1] nentries [2] status */
+	u32 mask;			/* capacity - 1 */
+	u32 arena_cap;
+};
+
 } /* namespace dng */
 
 struct dng_plan {

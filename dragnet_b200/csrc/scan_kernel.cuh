@@ -76,21 +76,6 @@ enum {
 
 enum { ST_TABLE_FULL = 1, ST_ARENA_FULL = 2 };
 
-struct GEntry {
-	unsigned long long tag;		/* 0 empty, else hash | 1 */
-	unsigned long long count;
-	u32 koff;			/* key offset in arena + 1; 0 = unpublished */
-	u32 klen;
-};
-
-struct GTable {
-	GEntry *entries;
-	u8 *arena;
-	u32 *misc;			/* [0] arena cursor [1] nentries [2] status */
-	u32 mask;			/* capacity - 1 */
-	u32 arena_cap;
-};
-
 /*
  * Per-CTA tally cache, two tiers (hashes pick the slot, key BYTES decide):
  *   tier 1: a few 64-byte slots with the key inline -- the common
