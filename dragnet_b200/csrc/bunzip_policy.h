@@ -18,8 +18,12 @@
 #include <stddef.h>
 #include <stdint.h>
 
+#ifndef DNG_BZ_WAVE_BLOCKS
 #define DNG_BZ_WAVE_BLOCKS ((size_t)1024)
+#endif
+#ifndef DNG_BZ_EMIT_OUT
 #define DNG_BZ_EMIT_OUT ((uint64_t)2 << 30)
+#endif
 
 namespace dng {
 

@@ -21,7 +21,9 @@
 #include <stdint.h>
 
 /* the smallest chunk, in compressed bytes */
+#ifndef DNG_GZ_SPLIT_FLOOR
 #define DNG_GZ_SPLIT_FLOOR ((uint64_t)64 << 10)
+#endif
 
 /* a chunk's decode must cover more than the window it reaches back over */
 static_assert(DNG_GZ_SPLIT_FLOOR >= 32768, "split floor below the window");
